@@ -1497,9 +1497,10 @@ __global__ void __launch_bounds__(128, MINB) event_tile_kernel(const __grid_cons
 // (tile kernel: 183 instructions per request but few warps per SM doing anything), and software pipelining costs registers and
 // bookkeeping instructions (440 per request, issue-bound).  The cheapest way to keep ≥ 64 KB per SM in flight is the hardware's own
 // warp scheduler: ONE request per warp, as many warps per SM as the register budget allows, a grid of ⌈requests / 8⌉ CTAs that the block
-// scheduler streams through the SMs.  Everything lives in registers: lane p holds the hash of block p, the two jump destinations are
-// probed by lanes 0 and last, a failed count test drains positions 1..last with one parallel probe per lane and an ordered ballot loop
-// (linear_scan_drain with the retain guard, event_tree.rs:582-657).  Only what needs the rolling prefix hashes or more than one jump
+// scheduler streams through the SMs.  Everything lives in registers: lane p owns block p.  Lanes 0 and last hash their blocks and probe
+// the two jump destinations; only a failed count test makes lanes 1..last-1 read and hash theirs, and then positions 1..last are drained
+// with one parallel probe per lane and an ordered ballot loop (linear_scan_drain with the retain guard, event_tree.rs:582-657).  A full
+// hit or a novel request thus reads 128 B of tokens, not all of them.  Only what needs the rolling prefix hashes or more than one jump
 // (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device queue and finished by event_slow_kernel right behind.
 struct SimpleLoc { uint32_t j, r; };
 __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t g) {
@@ -1511,7 +1512,7 @@ __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t 
 
 template <int MINB>
 __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
-                                                                  uint32_t* __restrict__ slow_queue, uint32_t pf_ahead) {
+                                                                  uint32_t* __restrict__ slow_queue) {
     __shared__ int32_t s_slice[64];
     __shared__ uint64_t s_load[64], s_ts[64];
     if (threadIdx.x < 64) {
@@ -1527,16 +1528,6 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
     const SimpleLoc loc = simple_locate(a, g);
     const BatchDesc& b = a.b[loc.j];
     const uint32_t off = __ldg(b.offsets + loc.r), ntok = __ldg(b.offsets + loc.r + 1) - off;
-    if (pf_ahead && g + pf_ahead < a.total && lane == 0) {
-        // pull the tokens of a request a couple of waves ahead into L2 (one bulk prefetch, fire and forget): the warp that will own it then
-        // starts its dependent chain with an L2 hit instead of a DRAM miss
-        const SimpleLoc lp = simple_locate(a, g + pf_ahead);
-        const BatchDesc& bp = a.b[lp.j];
-        const uint32_t po = __ldg(bp.offsets + lp.r), pe = __ldg(bp.offsets + lp.r + 1);
-        const uintptr_t lo = reinterpret_cast<uintptr_t>(bp.tokens + po) & ~(uintptr_t)15;
-        const uintptr_t hi = (reinterpret_cast<uintptr_t>(bp.tokens + pe) + 15) & ~(uintptr_t)15;
-        if (hi > lo && hi - lo <= (1u << 16)) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((uint32_t)(hi - lo)) : "memory");
-    }
     const FleetDerived* fd = f.derived;
     int32_t out = -1;
     uint32_t branch = SMGX_BR_NO_HEALTHY, matched = 0;
@@ -1553,11 +1544,11 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
                     return;
                 }
                 const int last = (int)nb - 1;
-                uint64_t h = 0;
-                if ((uint32_t)lane < nb) h = hash_block<16>(b.tokens + off + (size_t)lane * 16, 16);
+                // a block's content hash depends on that block alone, so only the two positions the jump search probes are hashed
+                // up front; the blocks in between are read only if the count test fails and the drain needs them
                 Slot sl{0, 0, SLOT_EMPTY, 0, 0};
                 bool found = false;
-                if (lane == 0 || lane == last) found = probe(v, (uint32_t)lane, h, sl);
+                if (lane == 0 || lane == last) found = probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
                 const uint64_t elig = f.elig[0];
                 uint64_t win = 0;
                 uint32_t score = 0;
@@ -1574,7 +1565,7 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
                             if (!bail && count != (uint32_t)__popcll(active)) {
                                 // linear_scan_drain over positions 1..=last (:582-657): every position probed at once, one lane each
                                 const bool in_range = lane >= 1 && lane <= last;
-                                if (lane >= 1 && lane < last) found = probe(v, (uint32_t)lane, h, sl);
+                                if (lane >= 1 && lane < last) found = probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
                                 const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
                                 uint64_t last_set = 0;
                                 uint32_t last_score = 0;
@@ -2017,11 +2008,9 @@ static int event_simple_minb() {   // SMGX_EVENT_SIMPLE=0|4|5|6: resident CTAs p
 }
 static void launch_simple(const EventIndexView& ix, const FleetView& fleet, const MultiArgs& a, int sm_count, cudaStream_t stream, uint32_t* d_queue, int minb) {
     const unsigned grid = (a.total + 7) / 8;
-    static const int pf_waves = [] { const char* e = getenv("SMGX_SIMPLE_PF"); return e ? atoi(e) : 0; }();   // waves of resident warps to prefetch ahead (0 = off)
-    const uint32_t pf_ahead = (uint32_t)std::max(pf_waves, 0) * 48u * (uint32_t)sm_count;
-    if (minb == 4) event_simple_kernel<4><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue, pf_ahead);
-    else if (minb == 6) event_simple_kernel<6><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue, pf_ahead);
-    else event_simple_kernel<5><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue, pf_ahead);
+    if (minb == 4) event_simple_kernel<4><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
+    else if (minb == 6) event_simple_kernel<6><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
+    else event_simple_kernel<5><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
     SMGX_CUDA(cudaGetLastError());
     const size_t smem = (size_t)std::max<uint32_t>(a.max_blocks, 1) * 8 * 8;
     if (smem > 48 * 1024) SMGX_CUDA(cudaFuncSetAttribute(event_slow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
