@@ -331,23 +331,40 @@ smgx_status smgx_select_batch_request_text(smgx_policy* p, const char* model_key
                                            int32_t* out_worker_idx, smgx_decision_info* out_info, char** err);
 
 /* ---- tokenizer: Tokenizer::encode for tiktoken-style models (crates/tokenizer/src/tiktoken.rs) ----------------- */
+/* The pre-tokenizer regex a tokenizer splits ordinary text with:
+ *   SMGX_PRETOK_CL100K  CL100K_BASE_PATTERN (tiktoken.rs:28): cl100k_base, and the Llama-3 Split regex of tokenizer.json files;
+ *   SMGX_PRETOK_R50K    tiktoken's GPT-2 pattern r50k_pat_str: r50k_base, p50k_base, p50k_edit, and tokenizer.json files whose
+ *                       pre-tokenizer is ByteLevel(use_regex = true, add_prefix_space = false) alone.
+ * Any other value is SMGX_INVALID_ARGUMENT. */
+typedef enum smgx_pretokenizer { SMGX_PRETOK_CL100K = 0, SMGX_PRETOK_R50K = 1 } smgx_pretokenizer;
 /* TiktokenTokenizer::from_file (tiktoken.rs:219-268): `path` holds lines of `base64(token) rank` (load_tiktoken_bpe, :346-367);
  * `special_strs/special_ids` = the added_tokens_decoder entries that become CoreBPE's special-token encoder (:234-238).
- * The pre-tokenizer is CL100K_BASE_PATTERN (:28).  One tokenizer per model key. */
+ * The pre-tokenizer is CL100K_BASE_PATTERN (:28); the _ex form takes it as an argument.  One tokenizer per model key, so one
+ * policy can hold models with different pre-tokenizers. */
 smgx_status smgx_tokenizer_load_tiktoken_file(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
                                               const uint32_t* special_ids, uint32_t n_special, char** err);
+smgx_status smgx_tokenizer_load_tiktoken_file_ex(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
+                                                 const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err);
 /* Same from memory: token i = blob[tok_offsets[i] .. tok_offsets[i+1]) with rank ranks[i]. */
 smgx_status smgx_tokenizer_load_tiktoken(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets,
                                          const uint32_t* ranks, uint32_t n_tokens, const char* const* special_strs,
                                          const uint32_t* special_ids, uint32_t n_special, char** err);
+smgx_status smgx_tokenizer_load_tiktoken_ex(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets,
+                                            const uint32_t* ranks, uint32_t n_tokens, const char* const* special_strs,
+                                            const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err);
 /* HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs:310-316 → crate `tokenizers`), byte-level BPE family whose tokenizer.json
- * has: no normalizer; pre_tokenizer = Split(Regex = the pattern above, Isolated) + ByteLevel(use_regex = false) — Llama 3 and kin;
+ * has: no normalizer; pre_tokenizer = Split(Regex = the cl100k pattern above, Isolated) + ByteLevel(use_regex = false) — Llama 3 and
+ * kin — or, with SMGX_PRETOK_R50K through the _ex form, ByteLevel(use_regex = true, add_prefix_space = false) alone — GPT-2 and kin;
  * model.type = "BPE" without dropout / unk / byte_fallback.  The caller parses the JSON (serde_json in the gateway,
  * smg_b200/policy.py here) and hands over: token i = blob[tok_offsets[i] .. tok_offsets[i+1]) as RAW bytes (byte-level chars mapped
  * back) with id ids[i]; `merges` = n_merges (left id, right id) pairs in priority order; model.ignore_merges; added_tokens as specials. */
 smgx_status smgx_tokenizer_load_bpe_merges(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
                                            uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges,
                                            const char* const* special_strs, const uint32_t* special_ids, uint32_t n_special, char** err);
+smgx_status smgx_tokenizer_load_bpe_merges_ex(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                              uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges,
+                                              const char* const* special_strs, const uint32_t* special_ids, uint32_t n_special,
+                                              smgx_pretokenizer pretokenizer, char** err);
 /* Encoder::encode_batch (tiktoken.rs:464-469) on the GPU: text i = text[offsets[i] .. offsets[i+1]) (UTF-8, already
  * chat-template-rendered; special-token strings are recognised, tiktoken.rs:446-460).  Writes the ragged token ids and
  * out_tok_offsets[n+1]; `cap_tokens` = capacity of out_tokens (≥ total text bytes is always enough). */

@@ -1,10 +1,11 @@
-// K1 — tokenize: the cl100k pre-tokenizer and tiktoken-style byte-pair merge as host+device functions.
+// K1 — tokenize: the cl100k and GPT-2 (r50k) pre-tokenizers and tiktoken-style byte-pair merge as host+device functions.
 //
 // Replaces, token for token, what the reference gets from the un-vendored crate tiktoken-rs through
 //   TiktokenTokenizer::encode → CoreBPE::encode_with_special_tokens   crates/tokenizer/src/tiktoken.rs:444-462
 // with the pattern CL100K_BASE_PATTERN (tiktoken.rs:28):
 //   (?i:'s|'t|'re|'ve|'m|'ll|'d) | [^\r\n\p{L}\p{N}]?\p{L}+ | \p{N}{1,3} | ?[^\s\p{L}\p{N}]+[\r\n]* | \s*[\r\n]+ | \s+(?!\S) | \s+
-// The regex is compiled by hand into next_piece_cl100k(): leftmost-first alternation, greedy quantifiers and the one
+// or with the GPT-2 pattern of r50k_base / p50k_base / p50k_edit (next_piece_r50k below).
+// Each regex is compiled by hand into a next_piece_*() function: leftmost-first alternation, greedy quantifiers and the one
 // backtracking look-ahead are resolved analytically (see the comments at each alternative).
 #pragma once
 #include <cstdint>
@@ -142,6 +143,95 @@ SMGX_HD uint32_t next_piece_cl100k(const uint8_t* s, uint32_t i, uint32_t n, con
     if (count >= 2) return last_start;     // 6.             : give back one char so that whitespace follows
     return j;                              // 7. \s+
 #undef SMGX_AT_END
+}
+
+// ---- GPT-2 / r50k pre-tokenizer ------------------------------------------------------------------------------------
+// tiktoken's r50k_pat_str (r50k_base, p50k_base, p50k_edit) and `tokenizers`' ByteLevel(use_regex = true), in the form
+//   's|'t|'re|'ve|'m|'ll|'d | ?\p{L}+ | ?\p{N}+ | ?[^\s\p{L}\p{N}]+ | \s+(?!\S) | \s+
+// Same contract as next_piece_cl100k.  Differences that matter: contractions are case-sensitive, digit runs are unbounded,
+// only U+0020 may lead a run, and there is no newline rule.
+enum class Pretok : uint8_t { Cl100k = 0, R50k = 1 };
+
+SMGX_HD bool is_contraction_tail(uint8_t b) {   // second byte of 's 't 'm 'd 're 've 'll
+    return b == 's' || b == 't' || b == 'm' || b == 'd' || b == 'r' || b == 'v' || b == 'l';
+}
+
+SMGX_HD uint32_t next_piece_r50k(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop = nullptr) {
+#define SMGX_AT_END(j) ((j) >= n || (stop != nullptr && stop[(j)] == 2))
+    uint32_t len0;
+    const uint32_t cp0 = utf8_decode(s, i, n, len0);
+    const uint8_t cls0 = char_class(cp0, u);
+
+    // 1. 's|'t|'re|'ve|'m|'ll|'d   (case-sensitive; the continuation bytes are ASCII, so bytes compare as characters)
+    if (cp0 == '\'' && !SMGX_AT_END(i + 1)) {
+        const uint8_t b1 = s[i + 1];
+        if (b1 == 's' || b1 == 't' || b1 == 'm' || b1 == 'd') return i + 2;
+        if ((b1 == 'r' || b1 == 'v' || b1 == 'l') && !SMGX_AT_END(i + 2)) {
+            const uint8_t b2 = s[i + 2];
+            if (b1 == 'l' ? b2 == 'l' : b2 == 'e') return i + 3;
+        }
+    }
+    // 2-4.  ?\p{L}+ |  ?\p{N}+ |  ?[^\s\p{L}\p{N}]+   — the three alternatives start with disjoint classes, so together they are
+    //      "a run of one non-space class, optionally led by one U+0020".  The space is taken only when a non-space follows it;
+    //      otherwise none of the three can match at i and the whitespace alternatives decide.
+    {
+        uint32_t j = i;
+        uint8_t rc = cls0;
+        if (cp0 == ' ' && !SMGX_AT_END(i + 1)) {
+            uint32_t l1;
+            const uint8_t c1 = char_class(utf8_decode(s, i + 1, n, l1), u);
+            if (c1 != CH_SPACE) { j = i + 1; rc = c1; }
+        }
+        if (rc != CH_SPACE) {
+            while (!SMGX_AT_END(j)) {
+                uint32_t l;
+                const uint32_t cp = utf8_decode(s, j, n, l);
+                if (char_class(cp, u) != rc) break;
+                j += l;
+            }
+            return j;
+        }
+    }
+    // 5-6. whitespace run starting at i (cls0 == CH_SPACE)
+    uint32_t j = i, last_start = i, count = 0;
+    while (!SMGX_AT_END(j)) {
+        uint32_t l;
+        const uint32_t cp = utf8_decode(s, j, n, l);
+        if (char_class(cp, u) != CH_SPACE) break;
+        last_start = j;
+        j += l;
+        ++count;
+    }
+    if (SMGX_AT_END(j)) return j;          // 5. \s+(?!\S) : run reaches the end of the (slice of) text
+    if (count >= 2) return last_start;     // 5.            : give back one char so that whitespace follows
+    return j;                              // 6. \s+        : a single whitespace char before a non-space
+#undef SMGX_AT_END
+}
+
+// Anchor rule of the r50k pattern: a piece certainly starts at p when the character before p is not whitespace and its class differs
+// from the class at p — unless that character is ' and the byte at p can continue a contraction.  `pc`/`pb` are the class and the
+// last byte of the previous character, `c`/`b` the class and the first byte of the character at p.  (Why it holds: DESIGN §4c.)
+SMGX_HD bool r50k_anchor_rule(uint8_t pc, uint8_t pb, uint8_t c, uint8_t b) {
+    if (pc == CH_SPACE || pc == c) return false;
+    return !(pb == '\'' && is_contraction_tail(b));
+}
+
+SMGX_HD uint32_t prev_cp(const uint8_t* s, uint32_t i, uint32_t lo) {   // code point ending right before byte i
+    uint32_t j = i - 1;
+    while (j > lo && (s[j] & 0xC0) == 0x80) --j;
+    uint32_t l;
+    return utf8_decode(s, j, i, l);
+}
+
+// Is byte i of the request s[beg..) (a lead byte, not inside a special) an r50k anchor?  `flags` (nullable) marks specials as in
+// next_piece_*: the byte after a special is an anchor, as is the request start.
+SMGX_HD bool is_anchor_r50k(const uint8_t* s, uint32_t i, uint32_t beg, const uint8_t* flags, const UnicodeView& u) {
+    if (i == beg) return true;
+    if (flags != nullptr && flags[i - 1] >= 2) return true;
+    uint32_t l;
+    const uint8_t c = char_class(utf8_decode(s, i, i + 4, l), u);   // valid UTF-8: a lead byte's continuation bytes exist
+    const uint8_t pc = char_class(prev_cp(s, i, beg), u);
+    return r50k_anchor_rule(pc, s[i - 1], c, s[i]);
 }
 
 // ---- vocabulary tables ---------------------------------------------------------------------------------------

@@ -1629,23 +1629,34 @@ static std::vector<std::pair<std::string, uint32_t>> collect_specials(const char
     for (uint32_t i = 0; i < n; ++i) { SMGX_REQUIRE(strs[i] != nullptr, "Invalid arguments: null pointer"); sp.emplace_back(strs[i], ids[i]); }
     return sp;
 }
-smgx_status smgx_tokenizer_load_tiktoken_file(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
-                                              const uint32_t* special_ids, uint32_t n_special, char** err) {
+// smgx_pretokenizer → Pretok; an unknown value is an invalid argument
+static Pretok pretok_of(smgx_pretokenizer pt) {
+    SMGX_REQUIRE(pt == SMGX_PRETOK_CL100K || pt == SMGX_PRETOK_R50K, "Invalid arguments: unknown pretokenizer " + std::to_string((int)pt));
+    return pt == SMGX_PRETOK_R50K ? Pretok::R50k : Pretok::Cl100k;
+}
+smgx_status smgx_tokenizer_load_tiktoken_file_ex(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
+                                                 const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {
     return guard(err, [&]() {
         NONNULL(p); NONNULL(path);
+        const Pretok pt = pretok_of(pretokenizer);
         std::lock_guard<std::mutex> g(p->impl.mu);
         bool dev = p->impl.cfg.device_id >= 0;
         if (dev) p->impl.use_device();
         ModelState& m = p->impl.model(model_key, true);
-        m.tokenizer.reset(Tokenizer::from_tiktoken_file(path, collect_specials(special_strs, special_ids, n_special), dev));
+        m.tokenizer.reset(Tokenizer::from_tiktoken_file(path, collect_specials(special_strs, special_ids, n_special), dev, pt));
         return SMGX_SUCCESS;
     });
 }
-smgx_status smgx_tokenizer_load_tiktoken(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets,
-                                         const uint32_t* ranks, uint32_t n_tokens, const char* const* special_strs,
-                                         const uint32_t* special_ids, uint32_t n_special, char** err) {
+smgx_status smgx_tokenizer_load_tiktoken_file(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
+                                              const uint32_t* special_ids, uint32_t n_special, char** err) {
+    return smgx_tokenizer_load_tiktoken_file_ex(p, model_key, path, special_strs, special_ids, n_special, SMGX_PRETOK_CL100K, err);
+}
+smgx_status smgx_tokenizer_load_tiktoken_ex(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets,
+                                            const uint32_t* ranks, uint32_t n_tokens, const char* const* special_strs,
+                                            const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {
     return guard(err, [&]() {
         NONNULL(p); NONNULL(blob); NONNULL(tok_offsets); NONNULL(ranks);
+        const Pretok pt = pretok_of(pretokenizer);
         std::lock_guard<std::mutex> g(p->impl.mu);
         bool dev = p->impl.cfg.device_id >= 0;
         if (dev) p->impl.use_device();
@@ -1653,17 +1664,29 @@ smgx_status smgx_tokenizer_load_tiktoken(smgx_policy* p, const char* model_key, 
         std::vector<uint32_t> rk(ranks, ranks + n_tokens);
         for (uint32_t i = 0; i < n_tokens; ++i) toks[i].assign((const char*)blob + tok_offsets[i], tok_offsets[i + 1] - tok_offsets[i]);
         ModelState& m = p->impl.model(model_key, true);
-        m.tokenizer.reset(new Tokenizer(toks, rk, collect_specials(special_strs, special_ids, n_special), dev));
+        m.tokenizer.reset(new Tokenizer(toks, rk, collect_specials(special_strs, special_ids, n_special), dev, pt));
         return SMGX_SUCCESS;
     });
+}
+smgx_status smgx_tokenizer_load_tiktoken(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets,
+                                         const uint32_t* ranks, uint32_t n_tokens, const char* const* special_strs,
+                                         const uint32_t* special_ids, uint32_t n_special, char** err) {
+    return smgx_tokenizer_load_tiktoken_ex(p, model_key, blob, tok_offsets, ranks, n_tokens, special_strs, special_ids, n_special, SMGX_PRETOK_CL100K, err);
 }
 
 smgx_status smgx_tokenizer_load_bpe_merges(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
                                            uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges, const char* const* special_strs,
                                            const uint32_t* special_ids, uint32_t n_special, char** err) {
+    return smgx_tokenizer_load_bpe_merges_ex(p, model_key, blob, tok_offsets, ids, n_tokens, merges, n_merges, ignore_merges, special_strs, special_ids,
+                                             n_special, SMGX_PRETOK_CL100K, err);
+}
+smgx_status smgx_tokenizer_load_bpe_merges_ex(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                              uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges, const char* const* special_strs,
+                                              const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {
     return guard(err, [&]() {
         NONNULL(p); NONNULL(blob); NONNULL(tok_offsets); NONNULL(ids);
         SMGX_REQUIRE(n_merges == 0 || merges, "Invalid arguments: null pointer");
+        const Pretok pt = pretok_of(pretokenizer);
         std::lock_guard<std::mutex> g(p->impl.mu);
         bool dev = p->impl.cfg.device_id >= 0;
         if (dev) p->impl.use_device();
@@ -1673,7 +1696,7 @@ smgx_status smgx_tokenizer_load_bpe_merges(smgx_policy* p, const char* model_key
         std::vector<std::pair<uint32_t, uint32_t>> mg(n_merges);
         for (uint32_t i = 0; i < n_merges; ++i) mg[i] = {merges[2 * i], merges[2 * i + 1]};
         ModelState& m = p->impl.model(model_key, true);
-        m.tokenizer.reset(new Tokenizer(toks, id, mg, ignore_merges != 0, collect_specials(special_strs, special_ids, n_special), dev));
+        m.tokenizer.reset(new Tokenizer(toks, id, mg, ignore_merges != 0, collect_specials(special_strs, special_ids, n_special), dev, pt));
         return SMGX_SUCCESS;
     });
 }

@@ -65,15 +65,10 @@ __global__ void __launch_bounds__(256) special_resolve_kernel(const uint32_t* __
 // alternative that consumes a letter stops at the end of the run or hands over to one that does), both ends of a digit
 // run (digits are consumed by \p{N}{1,3} only), the start of the request and the byte after a special — cut the text
 // into short independent segments; one thread per such "anchor" replays the hand-compiled regex until the next anchor
-// and appends every piece it finds to a dense piece list (CTA-staged, one global atomic per CTA).
+// and appends every piece it finds to a dense piece list (CTA-staged, one global atomic per CTA).  The r50k pattern has its
+// own anchor rule (bpe.cuh: r50k_anchor_rule); the cl100k one is wrong there (" 123" is one r50k piece).
 struct Piece { uint32_t start, len, req; };
 
-__device__ __forceinline__ uint32_t prev_cp(const uint8_t* s, uint32_t i, uint32_t lo) {   // code point ending right before byte i
-    uint32_t j = i - 1;
-    while (j > lo && (s[j] & 0xC0) == 0x80) --j;
-    uint32_t l;
-    return utf8_decode(s, j, i, l);
-}
 __device__ __forceinline__ bool is_anchor(const uint8_t* s, uint32_t i, uint32_t beg, const uint8_t* flags, const UnicodeView& u) {
     if (i == beg) return true;
     if (flags[i - 1] >= 2) return true;                      // byte after a special token
@@ -185,6 +180,61 @@ __device__ __forceinline__ uint32_t next_piece_window(const uint8_t* __restrict_
 #undef WIN_END
 }
 
+// Window form of next_piece_r50k, same contract as next_piece_window (kBail when a decision needs a byte beyond the window).
+__device__ __forceinline__ uint32_t next_piece_window_r50k(const uint8_t* __restrict__ s_txt, const uint8_t* __restrict__ s_cls, const uint8_t* __restrict__ s_stop,
+                                                           uint32_t k, uint32_t W, bool ends_text) {
+#define WIN_NEED(j) do { if ((j) >= W && !ends_text) return kBail; } while (0)
+#define WIN_END(j) ((j) >= W || s_stop[(j)])
+    const uint8_t c0 = s_cls[k] & 0x0F;
+    const uint8_t b0 = s_txt[k];
+    // 1. 's|'t|'re|'ve|'m|'ll|'d  (case-sensitive)
+    if (b0 == '\'') {
+        WIN_NEED(k + 1);
+        if (!WIN_END(k + 1)) {
+            const uint8_t b1 = s_txt[k + 1];
+            if (b1 == 's' || b1 == 't' || b1 == 'm' || b1 == 'd') return k + 2;
+            if (b1 == 'r' || b1 == 'v' || b1 == 'l') {
+                WIN_NEED(k + 2);
+                if (!WIN_END(k + 2) && (b1 == 'l' ? s_txt[k + 2] == 'l' : s_txt[k + 2] == 'e')) return k + 3;
+            }
+        }
+    }
+    // 2-4.  ?\p{L}+ |  ?\p{N}+ |  ?[^\s\p{L}\p{N}]+  — a run of one non-space class, optionally led by one U+0020
+    {
+        uint32_t j = k;
+        uint8_t rc = c0;
+        if (b0 == ' ') {
+            WIN_NEED(k + 1);
+            if (!WIN_END(k + 1) && (s_cls[k + 1] & 0x0F) != CH_SPACE) { j = k + 1; rc = s_cls[k + 1] & 0x0F; }
+        }
+        if (rc != CH_SPACE) {
+            for (;;) {
+                WIN_NEED(j);
+                if (WIN_END(j) || (s_cls[j] & 0x0F) != rc) break;
+                j += s_cls[j] >> 4;
+            }
+            return j;
+        }
+    }
+    // 5-6. whitespace run starting at k
+    uint32_t j = k, last_start = k, count = 0;
+    for (;;) {
+        WIN_NEED(j);
+        if (WIN_END(j) || (s_cls[j] & 0x0F) != CH_SPACE) break;
+        last_start = j;
+        j += s_cls[j] >> 4;
+        ++count;
+    }
+    if (WIN_END(j)) return j;              // 5. \s+(?!\S): the run reaches the end of the (slice of) text
+    if (count >= 2) return last_start;     // 5. give back one char so that whitespace follows
+    return j;                              // 6. \s+
+#undef WIN_NEED
+#undef WIN_END
+}
+
+// One kernel per pattern: the instantiations share the window classification, anchor packing and piece flush, and differ in the anchor
+// rule and the two matchers.
+template <Pretok P>
 __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
                                                           uint8_t* __restrict__ flags, Piece* __restrict__ pieces, uint32_t* __restrict__ n_pieces) {
     __shared__ Piece s_list[320];
@@ -220,7 +270,8 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
         while (q >= 0 && s_cls[q] == kCont) --q;
         if (q >= 0) pc = s_cls[q] & 0x0F;
         else pc = char_class(prev_cp(text, gi, beg), v.uni);
-        return (pc == CH_LETTER && c != CH_LETTER) || (c == CH_NUMBER) != (pc == CH_NUMBER);
+        if constexpr (P == Pretok::R50k) return r50k_anchor_rule(pc, k ? s_txt[k - 1] : text[gi - 1], c, s_txt[k]);
+        else return (pc == CH_LETTER && c != CH_LETTER) || (c == CH_NUMBER) != (pc == CH_NUMBER);
     };
     // phase 1: which bytes are anchors?  They are then packed densely, so that phase 2 — the serial regex replay — runs with full
     // warps instead of one live lane in six.
@@ -242,14 +293,23 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
             if (live) {
                 flags[p] = 1;
                 uint32_t q = kBail;
-                if (p - cstart < W) { const uint32_t e = next_piece_window(s_txt, s_cls, s_stop, p - cstart, W, ends_text); if (e != kBail) q = cstart + e; }
-                if (q == kBail) q = next_piece_cl100k(text, p, rend, v.uni, flags);   // the piece looks beyond the window
+                if (p - cstart < W) {
+                    uint32_t e;
+                    if constexpr (P == Pretok::R50k) e = next_piece_window_r50k(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
+                    else e = next_piece_window(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
+                    if (e != kBail) q = cstart + e;
+                }
+                if (q == kBail) {   // the piece looks beyond the window
+                    if constexpr (P == Pretok::R50k) q = next_piece_r50k(text, p, rend, v.uni, flags);
+                    else q = next_piece_cl100k(text, p, rend, v.uni, flags);
+                }
                 const uint32_t slot = atomicAdd(&s_count, 1u);
                 if (slot < 320) s_list[slot] = Piece{p, q - p, r};
                 else { const uint32_t g = atomicAdd(n_pieces, 1u); pieces[g] = Piece{p, q - p, r}; }   // overflow: straight to the global list
                 bool stop;
                 if (q >= rend) stop = true;
                 else if (q - cstart < W) stop = s_flag[q - cstart] == 2 || anchor_at(q - cstart);
+                else if constexpr (P == Pretok::R50k) stop = flags[q] == 2 || is_anchor_r50k(text, q, beg, flags, v.uni);
                 else stop = flags[q] == 2 || is_anchor(text, q, beg, flags, v.uni);
                 if (stop) live = false; else p = q;
             }
@@ -513,7 +573,8 @@ std::string b64decode(const std::string& in) {
 
 }  // namespace
 
-Tokenizer* Tokenizer::from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device) {
+Tokenizer* Tokenizer::from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device,
+                                          Pretok pretok) {
     // load_tiktoken_bpe (tiktoken.rs:346-367): lines of `base64(token) rank`
     std::ifstream f(path);
     if (!f) throw Error(SMGX_TOKENIZATION_ERROR, "cannot open tiktoken file '" + path + "'");
@@ -529,17 +590,17 @@ Tokenizer* Tokenizer::from_tiktoken_file(const std::string& path, const std::vec
         toks.push_back(b64decode(b64));
         ranks.push_back((uint32_t)std::stoul(rk));
     }
-    return new Tokenizer(toks, ranks, specials, device);
+    return new Tokenizer(toks, ranks, specials, device, pretok);
 }
 
 Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ranks,
-                     const std::vector<std::pair<std::string, uint32_t>>& specials, bool device)
-    : device_(device) {
+                     const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok)
+    : device_(device), pretok_(pretok) {
     build(tokens, ranks, nullptr, true, specials);
 }
 Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
-                     bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device)
-    : device_(device) {
+                     bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok)
+    : device_(device), pretok_(pretok) {
     build(tokens, ids, &merges, ignore_merges, specials);
 }
 
@@ -686,7 +747,10 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
         }
         SMGX_CUDA(cudaMemsetAsync(sc.n_pieces.ptr, 0, 16, stream));
         if (max_len) {
-            pretokenize_kernel<<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+            if (pretok_ == Pretok::R50k)
+                pretokenize_kernel<Pretok::R50k><<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+            else
+                pretokenize_kernel<Pretok::Cl100k><<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             ++*launches;
             // the piece count lives on the device, so the grids are sized for the worst case the text allows and stride over the lists

@@ -13,15 +13,16 @@ namespace smgx {
 
 class Tokenizer {
 public:
-    // tokens[i] = bytes of the vocab entry with rank/id ranks[i]; specials = (string, id)
+    // tokens[i] = bytes of the vocab entry with rank/id ranks[i]; specials = (string, id); pretok = the pre-tokenizer regex
     Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ranks,
-              const std::vector<std::pair<std::string, uint32_t>>& specials, bool device);
+              const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok);
     // HuggingFace `tokenizers` BPE (byte-level): merge priority = position in `merges` (pairs of ids), only listed pairs merge;
     // ignore_merges = look the whole piece up in the vocabulary first (models::bpe ignore_merges, Llama 3).
     Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
-              bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device);
+              bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok);
     ~Tokenizer();
-    static Tokenizer* from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device);
+    static Tokenizer* from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device,
+                                         Pretok pretok);
 
     BpeView view() const { return dview_; }
     uint32_t vocab_size() const { return vocab_size_; }
@@ -43,6 +44,7 @@ private:
     BpeView dview_{};
     uint32_t vocab_size_ = 0, n_pairs_ = 0;
     bool device_ = false;
+    Pretok pretok_ = Pretok::Cl100k;
     DevBuf d_byte_token_, d_pairs_, d_pieces_, d_blob_, d_specials_, d_uni_lo_, d_uni_hi_, d_uni_cls_;
 };
 

@@ -409,16 +409,24 @@ class Tree:
         return res
 
 
+# The reference's TiktokenModel set (tiktoken.rs:136-184) → the pre-tokenizer regex of the encoding.  r50k_base, p50k_base and
+# p50k_edit all split text with tiktoken's GPT-2 pattern; they differ only in vocabulary and specials, which the caller supplies.
+TIKTOKEN_ENCODINGS = {"cl100k_base": _lib.PRETOK_CL100K, "r50k_base": _lib.PRETOK_R50K, "p50k_base": _lib.PRETOK_R50K, "p50k_edit": _lib.PRETOK_R50K}
+
+
 class TiktokenTokenizer:
     """tokenizer::TiktokenTokenizer (crates/tokenizer/src/tiktoken.rs:132) on the GPU, bound to (policy handle, model).
-    encode() keeps the reference's behaviour of always recognising special-token strings (tiktoken.rs:444-462)."""
+    encode() keeps the reference's behaviour of always recognising special-token strings (tiktoken.rs:444-462).
+    `encoding` names the tiktoken encoding whose pre-tokenizer regex is used (TIKTOKEN_ENCODINGS)."""
 
-    def __init__(self, handle: _Handle, model: str, path: str, special_tokens=None):
+    def __init__(self, handle: _Handle, model: str, path: str, special_tokens=None, encoding: str = "cl100k_base"):
+        if encoding not in TIKTOKEN_ENCODINGS:
+            raise ValueError(f"unknown tiktoken encoding {encoding!r}; supported: {', '.join(TIKTOKEN_ENCODINGS)}")
         self.h, self.model = handle, model.encode()
         sp = list((special_tokens or {}).items())
         strs = (C.c_char_p * max(len(sp), 1))(*[k.encode() for k, _ in sp]) if sp else None
         ids = _u32([v for _, v in sp])
-        self.h.call("smgx_tokenizer_load_tiktoken_file", self.model, path.encode(), strs, _p(ids), len(sp))
+        self.h.call("smgx_tokenizer_load_tiktoken_file_ex", self.model, path.encode(), strs, _p(ids), len(sp), TIKTOKEN_ENCODINGS[encoding])
 
     @staticmethod
     def _ragged(texts):
@@ -456,10 +464,31 @@ def _byte_level_decoder():
     return {chr(c): b for b, c in zip(bs, cs)}
 
 
+def _hf_pretokenizer(pre):
+    """tokenizer.json `pre_tokenizer` → smgx_pretokenizer, or ValueError for a shape the GPU path does not implement.  Two shapes:
+    Split(Llama-3 / cl100k regex, Isolated) + ByteLevel(use_regex=False), and GPT-2's ByteLevel(use_regex=True, add_prefix_space=False)
+    alone or as a one-element Sequence (its built-in regex is tiktoken's r50k pattern)."""
+    steps = pre.get("pretokenizers", [pre]) if pre.get("type") == "Sequence" else [pre]
+    kinds = [s.get("type") for s in steps]
+    if kinds == ["ByteLevel"]:
+        bl = steps[0]
+        if bl.get("use_regex", True) is True and bl.get("add_prefix_space") is False:   # use_regex defaults to true in the crate
+            return _lib.PRETOK_R50K
+        raise ValueError("tokenizer.json: a lone ByteLevel pre_tokenizer must have use_regex=True and add_prefix_space=False")
+    split = [s for s in steps if s.get("type") == "Split"]
+    bl = [s for s in steps if s.get("type") == "ByteLevel"]
+    if kinds != ["Split", "ByteLevel"] or split[0].get("pattern", {}).get("Regex") != LLAMA3_SPLIT_PATTERN or \
+            str(split[0].get("behavior")).lower() != "isolated" or split[0].get("invert") or bl[0].get("use_regex") or bl[0].get("add_prefix_space"):
+        raise ValueError("tokenizer.json: pre_tokenizer must be Split(Llama-3 regex, Isolated) + ByteLevel(use_regex=False), "
+                         "or ByteLevel(use_regex=True, add_prefix_space=False) alone")
+    return _lib.PRETOK_CL100K
+
+
 class HuggingFaceTokenizer(TiktokenTokenizer):
     """tokenizer::HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs) for the byte-level BPE family the GPU path covers:
-    tokenizer.json with no normalizer, Split(Llama-3 / cl100k regex, Isolated) + ByteLevel(use_regex=False), model BPE without
-    dropout / unk / byte_fallback.  Anything else is refused loudly — there is no CPU tokenizer behind this."""
+    tokenizer.json with no normalizer, either Split(Llama-3 / cl100k regex, Isolated) + ByteLevel(use_regex=False) or GPT-2's
+    ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk / byte_fallback.  Anything else is
+    refused loudly — there is no CPU tokenizer behind this."""
 
     def __init__(self, handle: _Handle, model: str, path: str):   # noqa: D401 — does not call the tiktoken loader
         import json
@@ -471,14 +500,7 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
             raise ValueError("tokenizer.json: only plain byte-level BPE models are supported on the GPU path")
         if j.get("normalizer") is not None:
             raise ValueError("tokenizer.json: normalizers are not supported on the GPU path")
-        pre = j.get("pre_tokenizer") or {}
-        steps = pre.get("pretokenizers", [pre]) if pre.get("type") == "Sequence" else [pre]
-        kinds = [s.get("type") for s in steps]
-        split = [s for s in steps if s.get("type") == "Split"]
-        bl = [s for s in steps if s.get("type") == "ByteLevel"]
-        if kinds != ["Split", "ByteLevel"] or split[0].get("pattern", {}).get("Regex") != LLAMA3_SPLIT_PATTERN or \
-                str(split[0].get("behavior")).lower() != "isolated" or split[0].get("invert") or bl[0].get("use_regex") or bl[0].get("add_prefix_space"):
-            raise ValueError("tokenizer.json: pre_tokenizer must be Split(Llama-3 regex, Isolated) + ByteLevel(use_regex=False)")
+        pretok = _hf_pretokenizer(j.get("pre_tokenizer") or {})
         dec = _byte_level_decoder()
         vocab = mdl["vocab"]
         toks = [bytes(dec[c] for c in s) for s in vocab]
@@ -492,13 +514,17 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         blob = np.frombuffer(b"".join(toks), dtype=np.uint8).copy()
         added = [(a["content"], a["id"]) for a in j.get("added_tokens", [])]
         for a in j.get("added_tokens", []):
-            if a.get("lstrip") or a.get("rstrip") or a.get("single_word") or a.get("normalized"):
-                raise ValueError("tokenizer.json: added tokens with lstrip / rstrip / single_word / normalized are not supported")
+            if a.get("lstrip") or a.get("rstrip") or a.get("single_word"):
+                raise ValueError("tokenizer.json: added tokens with lstrip / rstrip / single_word are not supported")
+        # Without a normalizer, `tokenizers` extracts added tokens in one pass over the raw text whether they are marked normalized or
+        # not, as long as all of them carry the same mark; a mix splits the text in two passes, which the GPU path does not implement.
+        if len({bool(a.get("normalized", False)) for a in j.get("added_tokens", [])}) > 1:
+            raise ValueError("tokenizer.json: added tokens with mixed `normalized` values are not supported")
         strs = (C.c_char_p * max(len(added), 1))(*[k.encode() for k, _ in added]) if added else None
         sp_ids = _u32([v for _, v in added])
         mg = _u32(merges)
-        self.h.call("smgx_tokenizer_load_bpe_merges", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
-                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), len(added))
+        self.h.call("smgx_tokenizer_load_bpe_merges_ex", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
+                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), len(added), pretok)
 
 
 TREE_BATCH_MODES = {"sequential": 0, "snapshot": 1}   # smgx_tree_batch_mode (include/smgx.h)
@@ -685,8 +711,8 @@ class CacheAwarePolicy:
         self._h.call("smgx_set_tree_batch_mode", TREE_BATCH_MODES[mode])
 
     # -- tokenizer + text-in pick (the whole hot path on the device) ------------------------------------------------
-    def load_tiktoken_tokenizer(self, path: str, special_tokens=None, model: str = UNKNOWN_MODEL_ID) -> TiktokenTokenizer:
-        return TiktokenTokenizer(self._h, model, path, special_tokens)
+    def load_tiktoken_tokenizer(self, path: str, special_tokens=None, model: str = UNKNOWN_MODEL_ID, encoding: str = "cl100k_base") -> TiktokenTokenizer:
+        return TiktokenTokenizer(self._h, model, path, special_tokens, encoding)
 
     def load_hf_tokenizer(self, path: str, model: str = UNKNOWN_MODEL_ID) -> HuggingFaceTokenizer:
         return HuggingFaceTokenizer(self._h, model, path)
