@@ -1540,7 +1540,7 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
             out = fd->min_load_idx; branch = SMGX_BR_EVENT_MIN_LOAD;   // until an overlap is found
             if (nb > 0 && v.n_workers > 0) {
                 if (nb > 32 || nb - 1 > v.jump) {   // more than one jump / more blocks than lanes: the generic search
-                    if (lane == 0) slow_queue[1 + atomicAdd(slow_queue, 1u)] = g;
+                    if (lane == 0) slow_queue[2 + atomicAdd(slow_queue, 1u)] = g;
                     return;
                 }
                 const int last = (int)nb - 1;
@@ -1598,7 +1598,7 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
                     }
                 }
                 if (bail) {
-                    if (lane == 0) slow_queue[1 + atomicAdd(slow_queue, 1u)] = g;
+                    if (lane == 0) slow_queue[2 + atomicAdd(slow_queue, 1u)] = g;
                     return;
                 }
                 if (win) {
@@ -1631,7 +1631,7 @@ __global__ void __launch_bounds__(256) event_slow_kernel(const __grid_constant__
     const uint64_t elig = f.elig[0];
     const int32_t min_load_idx = f.derived->min_load_idx;
     for (uint32_t q = blockIdx.x * wpc + wic; q < n_slow; q += gridDim.x * wpc) {
-        const uint32_t g = slow_queue[1 + q];
+        const uint32_t g = slow_queue[2 + q];
         const SimpleLoc loc = simple_locate(a, g);
         const BatchDesc& b = a.b[loc.j];
         const uint32_t off = __ldg(b.offsets + loc.r), ntok = __ldg(b.offsets + loc.r + 1) - off;
@@ -1650,9 +1650,10 @@ __global__ void __launch_bounds__(256) event_slow_kernel(const __grid_constant__
         if (lane == 0) write_pick(b, loc.r, out, branch, matched, ntok);
         __syncwarp();
     }
-    // the last CTA out resets the queue for the next launch on this lane
+    // the last CTA out resets the count and the exit counter for the next launch on this lane; the counter sits at a fixed word, so a
+    // launch of another size still finds it at zero (the entries need no reset: only [2, 2 + count) is read)
     __syncthreads();
-    if (threadIdx.x == 0 && atomicAdd(slow_queue + a.total + 1, 1u) == gridDim.x - 1) { slow_queue[0] = 0; slow_queue[a.total + 1] = 0; }
+    if (threadIdx.x == 0 && atomicAdd(slow_queue + 1, 1u) == gridDim.x - 1) { slow_queue[0] = 0; slow_queue[1] = 0; }
 }
 
 // L2 prefetch of a request's token range, two pipeline stages ahead of its use: PF = 1 one bulk prefetch per request issued by lane 0

@@ -303,7 +303,7 @@ public:
         a.uniform_n = uniform && count ? descs[0].n : 0;
         a.hashes = nullptr;
         a.slow_queue = nullptr;
-        if (event_select_fused() && !cand_mode && !done_flag && rows > 0) {   // queue of the simple kernel (zeroed once; the slow kernel leaves it zeroed)
+        if (event_select_fused() && !cand_mode && !done_flag && rows > 0) {   // queue of the simple kernel (zeroed when allocated; the slow kernel leaves the count and exit counter zeroed)
             const size_t need = ((size_t)rows + 2) * 4;
             if (need > lane.d_slowq.cap) {
                 lane.d_slowq.reserve(need * 2);
