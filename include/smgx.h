@@ -334,9 +334,16 @@ smgx_status smgx_select_batch_request_text(smgx_policy* p, const char* model_key
 /* The pre-tokenizer regex a tokenizer splits ordinary text with:
  *   SMGX_PRETOK_CL100K  CL100K_BASE_PATTERN (tiktoken.rs:28): cl100k_base, and the Llama-3 Split regex of tokenizer.json files;
  *   SMGX_PRETOK_R50K    tiktoken's GPT-2 pattern r50k_pat_str: r50k_base, p50k_base, p50k_edit, and tokenizer.json files whose
- *                       pre-tokenizer is ByteLevel(use_regex = true, add_prefix_space = false) alone.
+ *                       pre-tokenizer is ByteLevel(use_regex = true, add_prefix_space = false) alone;
+ *   SMGX_PRETOK_QWEN2   the Qwen2 Split regex: the cl100k pattern with \p{N} in place of \p{N}{1,3} (every digit is a piece).
  * Any other value is SMGX_INVALID_ARGUMENT. */
-typedef enum smgx_pretokenizer { SMGX_PRETOK_CL100K = 0, SMGX_PRETOK_R50K = 1 } smgx_pretokenizer;
+typedef enum smgx_pretokenizer { SMGX_PRETOK_CL100K = 0, SMGX_PRETOK_R50K = 1, SMGX_PRETOK_QWEN2 = 2 } smgx_pretokenizer;
+/* The tokenizer.json normalizer applied to the text between special tokens before it is split:
+ *   SMGX_NORMALIZER_NONE  none;
+ *   SMGX_NORMALIZER_NFC   {"type": "NFC"} (Qwen2 and later), with the Unicode tables of the `tokenizers` crate.
+ * Special-token strings are matched on the raw text (added tokens with normalized = false).  Any other value is
+ * SMGX_INVALID_ARGUMENT. */
+typedef enum smgx_normalizer { SMGX_NORMALIZER_NONE = 0, SMGX_NORMALIZER_NFC = 1 } smgx_normalizer;
 /* TiktokenTokenizer::from_file (tiktoken.rs:219-268): `path` holds lines of `base64(token) rank` (load_tiktoken_bpe, :346-367);
  * `special_strs/special_ids` = the added_tokens_decoder entries that become CoreBPE's special-token encoder (:234-238).
  * The pre-tokenizer is CL100K_BASE_PATTERN (:28); the _ex form takes it as an argument.  One tokenizer per model key, so one
@@ -365,9 +372,15 @@ smgx_status smgx_tokenizer_load_bpe_merges_ex(smgx_policy* p, const char* model_
                                               uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges,
                                               const char* const* special_strs, const uint32_t* special_ids, uint32_t n_special,
                                               smgx_pretokenizer pretokenizer, char** err);
+/* The same with a normalizer (tokenizer.json `normalizer`); the _ex form forwards with SMGX_NORMALIZER_NONE. */
+smgx_status smgx_tokenizer_load_bpe_merges_norm(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                                uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges,
+                                                const char* const* special_strs, const uint32_t* special_ids, uint32_t n_special,
+                                                smgx_pretokenizer pretokenizer, smgx_normalizer normalizer, char** err);
 /* Encoder::encode_batch (tiktoken.rs:464-469) on the GPU: text i = text[offsets[i] .. offsets[i+1]) (UTF-8, already
  * chat-template-rendered; special-token strings are recognised, tiktoken.rs:446-460).  Writes the ragged token ids and
- * out_tok_offsets[n+1]; `cap_tokens` = capacity of out_tokens (≥ total text bytes is always enough). */
+ * out_tok_offsets[n+1]; `cap_tokens` = capacity of out_tokens: total text bytes is always enough for a tokenizer without a
+ * normalizer, 3 × total text bytes for a normalizing one (NFC can grow text threefold, e.g. U+1D160 → three code points). */
 smgx_status smgx_tokenize_batch(smgx_policy* p, const char* model_key, const uint8_t* text, const uint32_t* offsets, uint32_t n,
                                 uint32_t* out_tokens, uint32_t* out_tok_offsets, uint32_t cap_tokens, char** err);
 /* The whole hot path in one call: tokenize on the device → cache-aware pick; the token ids never visit the host unless

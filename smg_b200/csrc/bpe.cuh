@@ -54,7 +54,9 @@ SMGX_HD bool is_newline(uint32_t cp) { return cp == '\n' || cp == '\r'; }
 // End (byte index) of the regex match that starts at byte i of s[0..n).  i < n and i is not a slice end.
 // tiktoken runs the regex only on the ordinary text between two special tokens; `stop` (nullable) marks the first byte of
 // every special with the value 2, and such a byte acts as the end of the string (for the run scans and for `(?!\S)`).
-SMGX_HD uint32_t next_piece_cl100k(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop = nullptr) {
+// kDigits is the longest digit run of alternative 3: \p{N}{1,3} in cl100k / Llama 3, \p{N} in Qwen2 (next_piece_qwen2 below).
+template <int kDigits>
+SMGX_HD uint32_t next_piece_llama(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop) {
 #define SMGX_AT_END(j) ((j) >= n || (stop != nullptr && stop[(j)] == 2))
     uint32_t len0;
     const uint32_t cp0 = utf8_decode(s, i, n, len0);
@@ -96,10 +98,10 @@ SMGX_HD uint32_t next_piece_cl100k(const uint8_t* s, uint32_t i, uint32_t n, con
             return j;
         }
     }
-    // 3. \p{N}{1,3}
+    // 3. \p{N}{1,3}  (Qwen2: \p{N})
     if (cls0 == CH_NUMBER) {
         uint32_t j = i + len0;
-        for (int c = 1; c < 3 && !SMGX_AT_END(j); ++c) {
+        for (int c = 1; c < kDigits && !SMGX_AT_END(j); ++c) {
             uint32_t l;
             uint32_t cp = utf8_decode(s, j, n, l);
             if (char_class(cp, u) != CH_NUMBER) break;
@@ -144,13 +146,26 @@ SMGX_HD uint32_t next_piece_cl100k(const uint8_t* s, uint32_t i, uint32_t n, con
     return j;                              // 7. \s+
 #undef SMGX_AT_END
 }
+SMGX_HD uint32_t next_piece_cl100k(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop = nullptr) {
+    return next_piece_llama<3>(s, i, n, u, stop);
+}
+
+// ---- Qwen2 pre-tokenizer -------------------------------------------------------------------------------------------
+// The Split regex of the Qwen2 / Qwen2.5 / Qwen3 tokenizer.json files: the cl100k pattern with \p{N} in place of \p{N}{1,3},
+//   (?i:'s|'t|'re|'ve|'m|'ll|'d) | [^\r\n\p{L}\p{N}]?\p{L}+ | \p{N} | ?[^\s\p{L}\p{N}]+[\r\n]* | \s*[\r\n]+ | \s+(?!\S) | \s+
+// so every digit is a piece of its own.  Anchor rule: cl100k's, except that every digit and the character after every digit start a
+// piece (no other alternative can take a digit).
+SMGX_HD uint32_t next_piece_qwen2(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop = nullptr) {
+    return next_piece_llama<1>(s, i, n, u, stop);
+}
+SMGX_HD bool qwen2_anchor_rule(uint8_t pc, uint8_t c) { return (pc == CH_LETTER && c != CH_LETTER) || c == CH_NUMBER || pc == CH_NUMBER; }
 
 // ---- GPT-2 / r50k pre-tokenizer ------------------------------------------------------------------------------------
 // tiktoken's r50k_pat_str (r50k_base, p50k_base, p50k_edit) and `tokenizers`' ByteLevel(use_regex = true), in the form
 //   's|'t|'re|'ve|'m|'ll|'d | ?\p{L}+ | ?\p{N}+ | ?[^\s\p{L}\p{N}]+ | \s+(?!\S) | \s+
 // Same contract as next_piece_cl100k.  Differences that matter: contractions are case-sensitive, digit runs are unbounded,
 // only U+0020 may lead a run, and there is no newline rule.
-enum class Pretok : uint8_t { Cl100k = 0, R50k = 1 };
+enum class Pretok : uint8_t { Cl100k = 0, R50k = 1, Qwen2 = 2 };
 
 SMGX_HD bool is_contraction_tail(uint8_t b) {   // second byte of 's 't 'm 'd 're 've 'll
     return b == 's' || b == 't' || b == 'm' || b == 'd' || b == 'r' || b == 'v' || b == 'l';
@@ -232,6 +247,15 @@ SMGX_HD bool is_anchor_r50k(const uint8_t* s, uint32_t i, uint32_t beg, const ui
     const uint8_t c = char_class(utf8_decode(s, i, i + 4, l), u);   // valid UTF-8: a lead byte's continuation bytes exist
     const uint8_t pc = char_class(prev_cp(s, i, beg), u);
     return r50k_anchor_rule(pc, s[i - 1], c, s[i]);
+}
+// Same for the Qwen2 pattern (qwen2_anchor_rule).
+SMGX_HD bool is_anchor_qwen2(const uint8_t* s, uint32_t i, uint32_t beg, const uint8_t* flags, const UnicodeView& u) {
+    if (i == beg) return true;
+    if (flags != nullptr && flags[i - 1] >= 2) return true;
+    uint32_t l;
+    const uint8_t c = char_class(utf8_decode(s, i, i + 4, l), u);
+    const uint8_t pc = char_class(prev_cp(s, i, beg), u);
+    return qwen2_anchor_rule(pc, c);
 }
 
 // ---- vocabulary tables ---------------------------------------------------------------------------------------

@@ -1631,8 +1631,8 @@ static std::vector<std::pair<std::string, uint32_t>> collect_specials(const char
 }
 // smgx_pretokenizer → Pretok; an unknown value is an invalid argument
 static Pretok pretok_of(smgx_pretokenizer pt) {
-    SMGX_REQUIRE(pt == SMGX_PRETOK_CL100K || pt == SMGX_PRETOK_R50K, "Invalid arguments: unknown pretokenizer " + std::to_string((int)pt));
-    return pt == SMGX_PRETOK_R50K ? Pretok::R50k : Pretok::Cl100k;
+    SMGX_REQUIRE(pt == SMGX_PRETOK_CL100K || pt == SMGX_PRETOK_R50K || pt == SMGX_PRETOK_QWEN2, "Invalid arguments: unknown pretokenizer " + std::to_string((int)pt));
+    return pt == SMGX_PRETOK_R50K ? Pretok::R50k : pt == SMGX_PRETOK_QWEN2 ? Pretok::Qwen2 : Pretok::Cl100k;
 }
 smgx_status smgx_tokenizer_load_tiktoken_file_ex(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
                                                  const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {
@@ -1683,10 +1683,18 @@ smgx_status smgx_tokenizer_load_bpe_merges(smgx_policy* p, const char* model_key
 smgx_status smgx_tokenizer_load_bpe_merges_ex(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
                                               uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges, const char* const* special_strs,
                                               const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {
+    return smgx_tokenizer_load_bpe_merges_norm(p, model_key, blob, tok_offsets, ids, n_tokens, merges, n_merges, ignore_merges, special_strs, special_ids,
+                                               n_special, pretokenizer, SMGX_NORMALIZER_NONE, err);
+}
+smgx_status smgx_tokenizer_load_bpe_merges_norm(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                                uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges, const char* const* special_strs,
+                                                const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, smgx_normalizer normalizer,
+                                                char** err) {
     return guard(err, [&]() {
         NONNULL(p); NONNULL(blob); NONNULL(tok_offsets); NONNULL(ids);
         SMGX_REQUIRE(n_merges == 0 || merges, "Invalid arguments: null pointer");
         const Pretok pt = pretok_of(pretokenizer);
+        SMGX_REQUIRE(normalizer == SMGX_NORMALIZER_NONE || normalizer == SMGX_NORMALIZER_NFC, "Invalid arguments: unknown normalizer " + std::to_string((int)normalizer));
         std::lock_guard<std::mutex> g(p->impl.mu);
         bool dev = p->impl.cfg.device_id >= 0;
         if (dev) p->impl.use_device();
@@ -1696,7 +1704,8 @@ smgx_status smgx_tokenizer_load_bpe_merges_ex(smgx_policy* p, const char* model_
         std::vector<std::pair<uint32_t, uint32_t>> mg(n_merges);
         for (uint32_t i = 0; i < n_merges; ++i) mg[i] = {merges[2 * i], merges[2 * i + 1]};
         ModelState& m = p->impl.model(model_key, true);
-        m.tokenizer.reset(new Tokenizer(toks, id, mg, ignore_merges != 0, collect_specials(special_strs, special_ids, n_special), dev, pt));
+        m.tokenizer.reset(new Tokenizer(toks, id, mg, ignore_merges != 0, collect_specials(special_strs, special_ids, n_special), dev, pt,
+                                        normalizer == SMGX_NORMALIZER_NFC));
         return SMGX_SUCCESS;
     });
 }
@@ -1715,7 +1724,7 @@ static void tokenize_on_lane(Policy& P, ModelState& m, Lane& lane, const uint8_t
     lane.d_text.reserve(std::max<uint32_t>(total, 1) + 16);
     lane.d_offsets.reserve(((size_t)n + 1) * 4);
     lane.d_toff.reserve(((size_t)n + 1) * 4);
-    lane.d_tokens.reserve((size_t)std::max<uint32_t>(total, 1) * 4 + 16);
+    lane.d_tokens.reserve((size_t)std::max<uint32_t>(total, 1) * m.tokenizer->growth() * 4 + 16);   // NFC can grow the text threefold
     if (n == 0) return;
     if (total) SMGX_CUDA(cudaMemcpyAsync(lane.d_text.ptr, text + base, total, cudaMemcpyHostToDevice, lane.stream));
     SMGX_CUDA(cudaMemcpyAsync(lane.d_offsets.ptr, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, lane.stream));
@@ -1723,6 +1732,15 @@ static void tokenize_on_lane(Policy& P, ModelState& m, Lane& lane, const uint8_t
     m.tokenizer->encode_batch(lane.d_text.as<uint8_t>() - base, lane.d_offsets.as<uint32_t>(), n, base, total + base, mx, lane.d_tokens.as<uint32_t>(),
                               lane.d_toff.as<uint32_t>(), lane.tok_scratch, lane.stream, &P.launches);
 }
+
+// Token bound of the text-in pick for requests of at most mx bytes: mx without a normalizer (a byte is at most one token); with one,
+// growth() × mx capped at max_tokens_per_request — a request longer than that after normalization takes the device-side over-length
+// treatment (pick -1, branch 255, error flag) instead of a write past its hash row.
+static uint32_t text_token_bound(const Policy& P, const ModelState& m, uint32_t mx) {
+    const uint64_t b = (uint64_t)mx * m.tokenizer->growth();
+    return std::max<uint32_t>((uint32_t)std::min<uint64_t>(b, std::max<uint64_t>(mx, P.cfg.max_tokens_per_request)), 1);
+}
+static bool text_may_exceed(const Policy& P, const ModelState& m, uint32_t mx) { return (uint64_t)mx * m.tokenizer->growth() > P.cfg.max_tokens_per_request; }
 
 static void copy_tokens_out(Lane& lane, uint32_t n, uint32_t* out_tokens, uint32_t* out_tok_offsets, uint32_t cap_tokens) {
     std::vector<uint32_t> toff_local;
@@ -1798,8 +1816,9 @@ static smgx_status select_batch_text_once(smgx_policy* p, const char* model_key,
         }
         lane.d_out.reserve((size_t)n * 4);
         if (out_info) lane.d_info.reserve((size_t)n * sizeof(smgx_decision_info));
-        // a request of b bytes has at most b tokens → bounds the per-request hash row
-        P.enqueue_tokens(m, lane, lane.d_tokens.as<uint32_t>(), lane.d_toff.as<uint32_t>(), n, std::max<uint32_t>(mx, 1), lane.d_out.as<int32_t>(),
+        // a request of b bytes has at most growth() × b tokens → bounds the per-request hash row
+        const bool may_overflow = text_may_exceed(P, m, mx);
+        P.enqueue_tokens(m, lane, lane.d_tokens.as<uint32_t>(), lane.d_toff.as<uint32_t>(), n, text_token_bound(P, m, mx), lane.d_out.as<int32_t>(),
                          out_info ? lane.d_info.as<smgx_decision_info>() : nullptr);
         SMGX_CUDA(cudaMemcpyAsync(out_worker_idx, lane.d_out.ptr, (size_t)n * 4, cudaMemcpyDeviceToHost, lane.stream));
         if (out_info)
@@ -1809,6 +1828,14 @@ static smgx_status select_batch_text_once(smgx_policy* p, const char* model_key,
         for (uint32_t i = 0; i < n; ++i) {
             int32_t idx = out_worker_idx[i];
             if (idx >= 0 && (size_t)idx < m.processed.size()) ++m.processed[(size_t)idx];
+        }
+        if (may_overflow) {   // a request over max_tokens_per_request only after normalization: reported by this call, once
+            uint32_t flag = 0;
+            SMGX_CUDA(cudaMemcpy(&flag, P.d_err.ptr, 4, cudaMemcpyDeviceToHost));
+            if (flag == 1) {
+                SMGX_CUDA(cudaMemset(P.d_err.ptr, 0, 4));
+                throw Error(SMGX_INVALID_ARGUMENT, "a request exceeded max_tokens_per_request after normalization");
+            }
         }
         return SMGX_SUCCESS;
     });
@@ -2390,7 +2417,7 @@ smgx_status smgx_submit_text(smgx_policy* p, const char* model_key, const uint8_
         if (n) {
             lane.d_out.reserve((size_t)n * 4);
             if (out_info) lane.d_info.reserve((size_t)n * sizeof(smgx_decision_info));
-            P.enqueue_tokens(m, lane, lane.d_tokens.as<uint32_t>(), lane.d_toff.as<uint32_t>(), n, std::max<uint32_t>(mx, 1), lane.d_out.as<int32_t>(),
+            P.enqueue_tokens(m, lane, lane.d_tokens.as<uint32_t>(), lane.d_toff.as<uint32_t>(), n, text_token_bound(P, m, mx), lane.d_out.as<int32_t>(),
                              out_info ? lane.d_info.as<smgx_decision_info>() : nullptr);
             SMGX_CUDA(cudaMemcpyAsync(out_worker_idx, lane.d_out.ptr, (size_t)n * 4, cudaMemcpyDeviceToHost, lane.stream));
             if (out_info)

@@ -7,6 +7,7 @@
 #include <sstream>
 #include <unordered_map>
 
+#include "nfc_tables.h"
 #include "unicode_tables.h"
 
 namespace smgx {
@@ -82,8 +83,10 @@ __device__ __forceinline__ bool is_anchor(const uint8_t* s, uint32_t i, uint32_t
 // the regex then runs on classes instead of decoding and binary-searching every code point again.  Same alternatives, same order,
 // same analytic resolution of the look-ahead as next_piece_cl100k; whenever a decision needs a byte beyond the window (and the
 // window does not end the request) it returns kBail and the caller falls back to the global-memory matcher for that piece.
+// kDigits as in next_piece_llama: 3 for cl100k, 1 for Qwen2.
 constexpr uint8_t kCont = 0x0F;
 constexpr uint32_t kBail = 0xFFFFFFFFu;
+template <int kDigits>
 __device__ __forceinline__ uint32_t next_piece_window(const uint8_t* __restrict__ s_txt, const uint8_t* __restrict__ s_cls, const uint8_t* __restrict__ s_stop,
                                                       uint32_t k, uint32_t W, bool ends_text) {
 #define WIN_NEED(j) do { if ((j) >= W && !ends_text) return kBail; } while (0)
@@ -129,10 +132,10 @@ __device__ __forceinline__ uint32_t next_piece_window(const uint8_t* __restrict_
             return j;
         }
     }
-    // 3. \p{N}{1,3}
+    // 3. \p{N}{1,3}  (Qwen2: \p{N})
     if (c0 == CH_NUMBER) {
         uint32_t j = k + len0;
-        for (int c = 1; c < 3; ++c) {
+        for (int c = 1; c < kDigits; ++c) {
             WIN_NEED(j);
             if (WIN_END(j) || (s_cls[j] & 0x0F) != CH_NUMBER) break;
             j += s_cls[j] >> 4;
@@ -271,6 +274,7 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
         if (q >= 0) pc = s_cls[q] & 0x0F;
         else pc = char_class(prev_cp(text, gi, beg), v.uni);
         if constexpr (P == Pretok::R50k) return r50k_anchor_rule(pc, k ? s_txt[k - 1] : text[gi - 1], c, s_txt[k]);
+        else if constexpr (P == Pretok::Qwen2) return qwen2_anchor_rule(pc, c);
         else return (pc == CH_LETTER && c != CH_LETTER) || (c == CH_NUMBER) != (pc == CH_NUMBER);
     };
     // phase 1: which bytes are anchors?  They are then packed densely, so that phase 2 — the serial regex replay — runs with full
@@ -296,11 +300,13 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
                 if (p - cstart < W) {
                     uint32_t e;
                     if constexpr (P == Pretok::R50k) e = next_piece_window_r50k(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
-                    else e = next_piece_window(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
+                    else if constexpr (P == Pretok::Qwen2) e = next_piece_window<1>(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
+                    else e = next_piece_window<3>(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
                     if (e != kBail) q = cstart + e;
                 }
                 if (q == kBail) {   // the piece looks beyond the window
                     if constexpr (P == Pretok::R50k) q = next_piece_r50k(text, p, rend, v.uni, flags);
+                    else if constexpr (P == Pretok::Qwen2) q = next_piece_qwen2(text, p, rend, v.uni, flags);
                     else q = next_piece_cl100k(text, p, rend, v.uni, flags);
                 }
                 const uint32_t slot = atomicAdd(&s_count, 1u);
@@ -310,6 +316,7 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
                 if (q >= rend) stop = true;
                 else if (q - cstart < W) stop = s_flag[q - cstart] == 2 || anchor_at(q - cstart);
                 else if constexpr (P == Pretok::R50k) stop = flags[q] == 2 || is_anchor_r50k(text, q, beg, flags, v.uni);
+                else if constexpr (P == Pretok::Qwen2) stop = flags[q] == 2 || is_anchor_qwen2(text, q, beg, flags, v.uni);
                 else stop = flags[q] == 2 || is_anchor(text, q, beg, flags, v.uni);
                 if (stop) live = false; else p = q;
             }
@@ -547,6 +554,164 @@ __global__ void __launch_bounds__(256) compact_tokens_kernel(const uint32_t* __r
     }
 }
 
+// K1n: NFC normalization stage, only for a tokenizer loaded with a normalizer.  It runs after the specials are resolved on the RAW text
+// (added tokens with normalized = false) and before the pre-tokenizer, and writes a normalized ragged copy of the batch — text, flags
+// (2/3 of the specials carried over) and the specials' ids — that the pre-tokenizer, BPE and compaction then run on unchanged.
+// Grids are sized for the raw text; nothing comes back to the host (the normalized length stays on the device).
+//   nfc_check_kernel    thread per byte: does the request hold a code point that is not NFC-stable?  Most text does not (a clean
+//                       request is its own NFC and is copied as it is)
+//   nfc_segment_kernel  dirty requests, thread per byte: a segment starts at every NFC-stable code point, at the request start and
+//                       after a special; its thread normalizes it in a 32-entry buffer into norm_tmp (3 bytes per input byte),
+//                       or hands it to the long list; seg_len / chunk_sum / nlen collect the output lengths
+//   nfc_long_kernel     warp per long segment (thousands of marks are legal): lane 0 normalizes it in global scratch, canonical
+//                       ordering by a counting sort with the histogram in shared memory
+//   scan_counts_kernel  normalized request lengths → offsets of the normalized batch
+//   nfc_write_kernel    thread per byte: clean requests copy, dirty ones place every segment at (earlier chunks of the request +
+//                       exclusive scan within the chunk)
+constexpr uint32_t kNfcShort = 32;
+struct NfcLong { uint32_t start, end, req; };
+
+__global__ void __launch_bounds__(256) nfc_check_kernel(NfcView nv, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                        const uint8_t* __restrict__ flags, uint32_t* __restrict__ dirty) {
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t i = beg + blockIdx.x * blockDim.x + threadIdx.x;
+    if (beg + blockIdx.x * blockDim.x >= rend) return;   // CTA-uniform
+    bool bad = false;
+    if (i < rend && text[i] >= 0xCC && flags[i] < 2) {   // lead byte of a code point ≥ U+0300 (everything below is stable)
+        uint32_t l;
+        bad = !nfc_stable(nv, utf8_decode(text, i, rend, l));
+    }
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) dirty[r] = 1;
+}
+
+__device__ __forceinline__ uint32_t block_sum_256(uint32_t x, uint32_t* s_w) {
+    x = __reduce_add_sync(0xffffffffu, x);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = x;
+    __syncthreads();
+    uint32_t t = 0;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) t += s_w[w];
+    __syncthreads();
+    return t;
+}
+
+__global__ void __launch_bounds__(256) nfc_segment_kernel(NfcView nv, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                          uint32_t first_byte, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ dirty,
+                                                          uint32_t* __restrict__ seg_len, uint32_t* __restrict__ chunk_sum, uint32_t* __restrict__ nlen,
+                                                          uint8_t* __restrict__ norm_tmp, NfcLong* __restrict__ longs, uint32_t* __restrict__ n_long) {
+    __shared__ uint32_t s_w[8];
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t cstart = beg + blockIdx.x * blockDim.x;
+    if (cstart >= rend) return;
+    if (!dirty[r]) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) nlen[r] = rend - beg;
+        return;
+    }
+    const uint32_t i = cstart + threadIdx.x;
+    uint32_t len = 0;
+    if (i < rend) {
+        const uint8_t fl = flags[i];
+        if (fl >= 2) len = 1;   // special-token byte: copied as it is
+        else if ((text[i] & 0xC0) != 0x80) {
+            uint32_t l;
+            const uint32_t cp = utf8_decode(text, i, rend, l);
+            const bool stable = nfc_stable(nv, cp);
+            if (stable || i == beg || flags[i - 1] >= 2) {
+                const uint32_t e = nfc_segment_end(nv, text, i, rend, flags);
+                uint8_t* out = norm_tmp + 3ull * (i - first_byte);
+                if (stable && e == i + l) {   // a stable code point alone is its own NFC
+                    for (uint32_t j = 0; j < l; ++j) out[j] = text[i + j];
+                    len = l;
+                } else {
+                    uint32_t ent[kNfcShort];
+                    uint32_t m = nfc_decompose_text(nv, text, i, e, ent, kNfcShort);
+                    if (m <= kNfcShort) {
+                        m = nfc_reorder_compose(nv, ent, m, nullptr, nullptr);
+                        len = nfc_encode(ent, m, out);
+                    } else {
+                        longs[atomicAdd(n_long, 1u)] = NfcLong{i, e, r};
+                    }
+                }
+            }
+        }
+        seg_len[i - first_byte] = len;
+    }
+    const uint32_t sum = block_sum_256(len, s_w);
+    if (threadIdx.x == 0) {
+        chunk_sum[cstart - first_byte] = sum;
+        if (sum) atomicAdd(&nlen[r], sum);
+    }
+}
+
+__global__ void __launch_bounds__(256) nfc_long_kernel(NfcView nv, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                       uint32_t first_byte, const NfcLong* __restrict__ longs, const uint32_t* __restrict__ n_long,
+                                                       uint32_t* __restrict__ ent, uint32_t* __restrict__ seg_len, uint32_t* __restrict__ chunk_sum,
+                                                       uint32_t* __restrict__ nlen, uint8_t* __restrict__ norm_tmp) {
+    __shared__ uint32_t s_hist[8][256];
+    const uint32_t n = *n_long;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t nw = gridDim.x * (blockDim.x >> 5);
+    for (uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += nw) {
+        if (lane != 0) continue;
+        const NfcLong sg = longs[k];
+        const uint64_t rel = sg.start - first_byte;
+        const uint32_t cap = 2 * (sg.end - sg.start);   // at most two code points per byte (the generator asserts it)
+        uint32_t* e = ent + 4 * rel;                     // [0, cap) the entries, [cap, 2 cap) the counting sort's buffer
+        uint32_t m = nfc_decompose_text(nv, text, sg.start, sg.end, e, cap);
+        m = nfc_reorder_compose(nv, e, m, e + cap, s_hist[wid]);
+        const uint32_t len = nfc_encode(e, m, norm_tmp + 3 * rel);
+        seg_len[rel] = len;
+        const uint32_t beg = offsets[sg.req];
+        atomicAdd(&chunk_sum[beg + (sg.start - beg) / 256 * 256 - first_byte], len);
+        atomicAdd(&nlen[sg.req], len);
+    }
+}
+
+__global__ void __launch_bounds__(256) nfc_write_kernel(const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets, uint32_t first_byte,
+                                                        const uint8_t* __restrict__ flags, const uint32_t* __restrict__ tmp_ids,
+                                                        const uint32_t* __restrict__ dirty, const uint32_t* __restrict__ seg_len,
+                                                        const uint32_t* __restrict__ chunk_sum, const uint8_t* __restrict__ norm_tmp,
+                                                        const uint32_t* __restrict__ noff, uint8_t* __restrict__ ntext, uint8_t* __restrict__ nflags,
+                                                        uint32_t* __restrict__ nids) {
+    __shared__ uint32_t s_w[8];
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t cstart = beg + blockIdx.x * blockDim.x;
+    if (cstart >= rend) return;
+    const uint32_t i = cstart + threadIdx.x;
+    const uint32_t out0 = noff[r];
+    if (!dirty[r]) {
+        if (i < rend) {
+            const uint32_t o = out0 + (i - beg);
+            const uint8_t fl = flags[i];
+            ntext[o] = text[i];
+            nflags[o] = fl;
+            if (fl >= 2) nids[o] = tmp_ids[i];
+        }
+        return;
+    }
+    uint32_t pre = 0;   // output bytes of the request's earlier chunks
+    for (uint32_t c = threadIdx.x; c < blockIdx.x; c += blockDim.x) pre += chunk_sum[beg + c * 256 - first_byte];
+    const uint32_t base = block_sum_256(pre, s_w);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t len = i < rend ? seg_len[i - first_byte] : 0;
+    uint32_t inc = len;   // inclusive scan within the warp, then across the 8 warps
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
+    if (lane == 31) s_w[wid] = inc;
+    __syncthreads();
+    uint32_t before = 0;
+    for (int w = 0; w < wid; ++w) before += s_w[w];
+    if (len) {
+        const uint32_t o = out0 + base + before + inc - len;
+        const uint8_t fl = flags[i];
+        if (fl >= 2) { ntext[o] = text[i]; nflags[o] = fl; nids[o] = tmp_ids[i]; }
+        else {
+            const uint8_t* src = norm_tmp + 3ull * (i - first_byte);
+            for (uint32_t j = 0; j < len; ++j) { ntext[o + j] = src[j]; nflags[o + j] = 0; }
+        }
+    }
+}
+
 uint32_t pow2_at_least(uint64_t x) { uint32_t p = 1024; while (p < x) p <<= 1; return p; }
 
 std::string b64decode(const std::string& in) {
@@ -599,8 +764,8 @@ Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<u
     build(tokens, ranks, nullptr, true, specials);
 }
 Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
-                     bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok)
-    : device_(device), pretok_(pretok) {
+                     bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok, bool nfc)
+    : device_(device), pretok_(pretok), nfc_(nfc) {
     build(tokens, ids, &merges, ignore_merges, specials);
 }
 
@@ -710,24 +875,47 @@ void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<
     dview_.n_special = (uint32_t)sp.size();
     for (int i = 0; i < 8; ++i) dview_.special_first[i] = first_bits[i];
     dview_.uni = UnicodeView{d_uni_lo_.as<uint32_t>(), d_uni_hi_.as<uint32_t>(), d_uni_cls_.as<uint8_t>(), kUniRanges};
+    if (nfc_) {   // the NFC tables, one allocation (every array 16-byte aligned)
+        std::vector<uint8_t> t;
+        auto put = [&t](const void* src, size_t bytes) {
+            const size_t at = (t.size() + 15) / 16 * 16;
+            t.resize(at + bytes);
+            memcpy(t.data() + at, src, bytes);
+            return at;
+        };
+        const size_t o_ccp = put(kNfcCccCp, sizeof(kNfcCccCp)), o_cv = put(kNfcCccVal, sizeof(kNfcCccVal));
+        const size_t o_dcp = put(kNfcDecCp, sizeof(kNfcDecCp)), o_doff = put(kNfcDecOff, sizeof(kNfcDecOff)), o_dd = put(kNfcDecData, sizeof(kNfcDecData));
+        const size_t o_ck = put(kNfcCompKey, sizeof(kNfcCompKey)), o_cval = put(kNfcCompVal, sizeof(kNfcCompVal));
+        const size_t o_ulo = put(kNfcUnstLo, sizeof(kNfcUnstLo)), o_uhi = put(kNfcUnstHi, sizeof(kNfcUnstHi));
+        up(d_nfc_, t.data(), t.size());
+        const uint8_t* b = d_nfc_.as<uint8_t>();
+        nview_ = NfcView{(const uint32_t*)(b + o_ccp), b + o_cv, kNfcCccN, (const uint32_t*)(b + o_dcp), (const uint16_t*)(b + o_doff),
+                         (const uint32_t*)(b + o_dd), kNfcDecN, (const uint64_t*)(b + o_ck), (const uint32_t*)(b + o_cval), kNfcCompN,
+                         (const uint32_t*)(b + o_ulo), (const uint32_t*)(b + o_uhi), kNfcUnstableN};
+    }
 }
 
 Tokenizer::~Tokenizer() {
     d_byte_token_.release(); d_pairs_.release(); d_pieces_.release(); d_blob_.release(); d_specials_.release();
-    d_uni_lo_.release(); d_uni_hi_.release(); d_uni_cls_.release();
+    d_uni_lo_.release(); d_uni_hi_.release(); d_uni_cls_.release(); d_nfc_.release();
 }
 
 void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, uint32_t n, uint32_t first_byte, uint32_t total_bytes, uint32_t max_len,
                              uint32_t* d_tokens, uint32_t* d_tok_offsets, Scratch& sc, cudaStream_t stream, uint64_t* launches) const {
     if (!device_) throw Error(SMGX_DEVICE_ERROR, "tokenizer was loaded without a device (host-mirror policy): no GPU path, no CPU fallback");
     if (n == 0) return;
+    const uint32_t raw = total_bytes - first_byte;
+    if (nfc_) SMGX_REQUIRE(3ull * raw < (1ull << 31) && 3ull * max_len < (1ull << 31), "text batch too large for the normalizer");
+    // bytes the pre-tokenizer and BPE see: the raw text, or its normalized copy (at most 3x, at absolute offsets from 0)
+    const uint32_t span = nfc_ ? 3 * raw : raw;
+    const uint32_t span_end = nfc_ ? span : total_bytes;
     sc.flags.reserve(std::max<uint32_t>(total_bytes, 1));
     sc.tmp_ids.reserve((size_t)std::max<uint32_t>(total_bytes, 1) * 4);
-    sc.tmp_rk.reserve((size_t)std::max<uint32_t>(total_bytes, 1) * 8);
+    sc.tmp_rk.reserve((size_t)std::max<uint32_t>(std::max(total_bytes, span_end), 1) * 8);
     sc.totals.reserve((size_t)n * 4);
-    sc.pieces.reserve((size_t)std::max<uint32_t>(total_bytes - first_byte, 1) * sizeof(Piece));
+    sc.pieces.reserve((size_t)std::max<uint32_t>(span, 1) * sizeof(Piece));
     sc.n_pieces.reserve(16);
-    sc.miss.reserve(((size_t)std::max<uint32_t>(total_bytes - first_byte, 1) + 1) * 8);
+    sc.miss.reserve(((size_t)std::max<uint32_t>(span, 1) + 1) * 8);
     if (total_bytes) {
         SMGX_CUDA(cudaMemsetAsync(sc.flags.ptr, 0, total_bytes, stream));
     }
@@ -745,34 +933,81 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
         } else {
             SMGX_CUDA(cudaMemsetAsync(sc.totals.ptr, 0, (size_t)n * 4, stream));
         }
+        // what the pre-tokenizer, BPE and compaction run on
+        const uint8_t* text = d_text;
+        const uint32_t* offsets = d_offsets;
+        uint8_t* flags = sc.flags.as<uint8_t>();
+        uint32_t* tmp_ids = sc.tmp_ids.as<uint32_t>();
+        uint32_t len_bound = max_len;
+        if (nfc_ && max_len) {
+            // scratch, 16-byte aligned slices of one allocation: normalized text / flags / ids (3 per raw byte), segment lengths and
+            // chunk sums (per raw byte), segment output (3 bytes per raw byte), long-segment entries (4 per raw byte), the long list,
+            // and per request: dirty, normalized length, normalized offsets; then the long count
+            const size_t R = std::max<uint32_t>(raw, 1);
+            size_t at = 0;
+            auto slice = [&at](size_t bytes) { const size_t o = at; at = (at + bytes + 15) / 16 * 16; return o; };
+            const size_t o_text = slice(3 * R), o_flags = slice(3 * R), o_ids = slice(3 * R * 4), o_seg = slice(R * 4), o_chunk = slice(R * 4),
+                         o_tmp = slice(3 * R), o_ent = slice(4 * R * 4), o_long = slice((R / 16 + 1) * sizeof(NfcLong)), o_req = slice(((size_t)3 * n + 1) * 4),
+                         o_cnt = slice(16);
+            sc.nfc.reserve(at);
+            uint8_t* b = sc.nfc.as<uint8_t>();
+            uint32_t* dirty = (uint32_t*)(b + o_req);
+            uint32_t* nlen = dirty + n;
+            uint32_t* noff = nlen + n;
+            uint32_t* n_long = (uint32_t*)(b + o_cnt);
+            SMGX_CUDA(cudaMemsetAsync(dirty, 0, (size_t)n * 8, stream));   // dirty and nlen
+            SMGX_CUDA(cudaMemsetAsync(n_long, 0, 16, stream));
+            // the raw-coordinate arrays are indexed from first_byte
+            uint32_t* seg_len = (uint32_t*)(b + o_seg);
+            uint32_t* chunk_sum = (uint32_t*)(b + o_chunk);
+            uint8_t* norm_tmp = b + o_tmp;
+            NfcLong* longs = (NfcLong*)(b + o_long);
+            nfc_check_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, flags, dirty);
+            nfc_segment_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, first_byte, flags, dirty, seg_len, chunk_sum, nlen, norm_tmp, longs, n_long);
+            const unsigned sms = current_sm_count();
+            nfc_long_kernel<<<sms, 256, 0, stream>>>(nview_, d_text, d_offsets, first_byte, longs, n_long, (uint32_t*)(b + o_ent), seg_len, chunk_sum, nlen, norm_tmp);
+            scan_counts_kernel<<<1, 1024, 0, stream>>>(nlen, n, noff);
+            nfc_write_kernel<<<grid2, 256, 0, stream>>>(d_text, d_offsets, first_byte, flags, tmp_ids, dirty, seg_len, chunk_sum, norm_tmp, noff,
+                                                        b + o_text, b + o_flags, (uint32_t*)(b + o_ids));
+            SMGX_CUDA(cudaGetLastError());
+            *launches += 5;
+            text = b + o_text;
+            offsets = noff;
+            flags = b + o_flags;
+            tmp_ids = (uint32_t*)(b + o_ids);
+            len_bound = 3 * max_len;
+        }
         SMGX_CUDA(cudaMemsetAsync(sc.n_pieces.ptr, 0, 16, stream));
         if (max_len) {
+            const dim3 gridp((len_bound + 255) / 256, n);   // with NFC: CTAs past a request's normalized end find an empty window
             if (pretok_ == Pretok::R50k)
-                pretokenize_kernel<Pretok::R50k><<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::R50k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+            else if (pretok_ == Pretok::Qwen2)
+                pretokenize_kernel<Pretok::Qwen2><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             else
-                pretokenize_kernel<Pretok::Cl100k><<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::Cl100k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             ++*launches;
             // the piece count lives on the device, so the grids are sized for the worst case the text allows and stride over the lists
             const unsigned sms = current_sm_count();
-            const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)(total_bytes - first_byte) / 2 + 255) / 256 + 1, sms * 16ull);
+            const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)span / 2 + 255) / 256 + 1, sms * 16ull);
             uint32_t* cnt = sc.n_pieces.as<uint32_t>();
             uint32_t* miss_short = sc.miss.as<uint32_t>();
-            uint32_t* miss_long = miss_short + (total_bytes - first_byte) + 1;
-            bpe_lookup_kernel<<<grid, 256, 0, stream>>>(dview_, d_text, sc.pieces.as<Piece>(), cnt, sc.tmp_ids.as<uint32_t>(), sc.totals.as<uint32_t>(), miss_short, miss_long);
-            bpe_merge_kernel<<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, d_text, sc.pieces.as<Piece>(), cnt, miss_short, sc.tmp_ids.as<uint32_t>(), sc.totals.as<uint32_t>());
-            bpe_long_kernel<<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, d_text, sc.pieces.as<Piece>(), cnt, miss_long, sc.tmp_ids.as<uint32_t>(),
+            uint32_t* miss_long = miss_short + span + 1;
+            bpe_lookup_kernel<<<grid, 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, tmp_ids, sc.totals.as<uint32_t>(), miss_short, miss_long);
+            bpe_merge_kernel<<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_short, tmp_ids, sc.totals.as<uint32_t>());
+            bpe_long_kernel<<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_long, tmp_ids,
                                                                     sc.tmp_rk.as<uint64_t>(), sc.totals.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             *launches += 3;
         }
+        scan_counts_kernel<<<1, 1024, 0, stream>>>(sc.totals.as<uint32_t>(), n, d_tok_offsets);
+        SMGX_CUDA(cudaGetLastError());
+        ++*launches;
+        compact_tokens_kernel<<<(unsigned)(((uint64_t)n * 32 + 255) / 256), 256, 0, stream>>>(offsets, n, tmp_ids, d_tok_offsets, d_tokens);
+        SMGX_CUDA(cudaGetLastError());
+        ++*launches;
     }
-    scan_counts_kernel<<<1, 1024, 0, stream>>>(sc.totals.as<uint32_t>(), n, d_tok_offsets);
-    SMGX_CUDA(cudaGetLastError());
-    ++*launches;
-    compact_tokens_kernel<<<(unsigned)(((uint64_t)n * 32 + 255) / 256), 256, 0, stream>>>(d_offsets, n, sc.tmp_ids.as<uint32_t>(), d_tok_offsets, d_tokens);
-    SMGX_CUDA(cudaGetLastError());
-    ++*launches;
 }
 
 }  // namespace smgx

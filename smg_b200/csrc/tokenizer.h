@@ -8,6 +8,7 @@
 
 #include "bpe.cuh"
 #include "common.h"
+#include "nfc.cuh"
 
 namespace smgx {
 
@@ -18,8 +19,9 @@ public:
               const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok);
     // HuggingFace `tokenizers` BPE (byte-level): merge priority = position in `merges` (pairs of ids), only listed pairs merge;
     // ignore_merges = look the whole piece up in the vocabulary first (models::bpe ignore_merges, Llama 3).
+    // nfc: the tokenizer.json normalizer is NFC (nfc.cuh); the text between specials is normalized before it is split.
     Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
-              bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok);
+              bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok, bool nfc = false);
     ~Tokenizer();
     static Tokenizer* from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device,
                                          Pretok pretok);
@@ -27,12 +29,14 @@ public:
     BpeView view() const { return dview_; }
     uint32_t vocab_size() const { return vocab_size_; }
     uint32_t n_pairs() const { return n_pairs_; }
+    // Most bytes of normalized text (and so most tokens) per byte of input: 3 with NFC (U+1D160 → three code points), else 1.
+    uint32_t growth() const { return nfc_ ? 3u : 1u; }
 
-    // Scratch needed for a batch of `total_bytes` of text and `n` requests.
-    struct Scratch { DevBuf flags, tmp_ids, tmp_rk, totals, pieces, n_pieces, miss; };
+    // Scratch needed for a batch of `total_bytes` of text and `n` requests; `nfc` holds the normalization stage's buffers.
+    struct Scratch { DevBuf flags, tmp_ids, tmp_rk, totals, pieces, n_pieces, miss, nfc; };
 
-    // Enqueue pre-tokenise + BPE + compaction on `stream`.
-    //   d_text/d_offsets (n+1): ragged UTF-8; d_tokens: capacity ≥ total_bytes u32; d_tok_offsets: n+1 u32 (written).
+    // Enqueue [NFC +] pre-tokenise + BPE + compaction on `stream`.
+    //   d_text/d_offsets (n+1): ragged UTF-8; d_tokens: capacity ≥ growth() × (total_bytes - first_byte) u32; d_tok_offsets: n+1 u32 (written).
     // Text bytes live at d_text[first_byte .. total_bytes) (absolute offsets as given in d_offsets).
     // `max_len` = longest request in bytes (sizes the 2-D grids).
     void encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, uint32_t n, uint32_t first_byte, uint32_t total_bytes, uint32_t max_len,
@@ -45,7 +49,9 @@ private:
     uint32_t vocab_size_ = 0, n_pairs_ = 0;
     bool device_ = false;
     Pretok pretok_ = Pretok::Cl100k;
-    DevBuf d_byte_token_, d_pairs_, d_pieces_, d_blob_, d_specials_, d_uni_lo_, d_uni_hi_, d_uni_cls_;
+    bool nfc_ = false;
+    NfcView nview_{};
+    DevBuf d_byte_token_, d_pairs_, d_pieces_, d_blob_, d_specials_, d_uni_lo_, d_uni_hi_, d_uni_cls_, d_nfc_;
 };
 
 }  // namespace smgx

@@ -423,6 +423,7 @@ class TiktokenTokenizer:
         if encoding not in TIKTOKEN_ENCODINGS:
             raise ValueError(f"unknown tiktoken encoding {encoding!r}; supported: {', '.join(TIKTOKEN_ENCODINGS)}")
         self.h, self.model = handle, model.encode()
+        self.growth = 1   # most tokens per byte of text: smgx_tokenize_batch's cap_tokens rule
         sp = list((special_tokens or {}).items())
         strs = (C.c_char_p * max(len(sp), 1))(*[k.encode() for k, _ in sp]) if sp else None
         ids = _u32([v for _, v in sp])
@@ -439,7 +440,7 @@ class TiktokenTokenizer:
     def encode_batch(self, texts, add_special_tokens: bool = False):
         data, offsets = self._ragged(texts)
         n = len(texts)
-        cap = int(offsets[-1]) + 1
+        cap = self.growth * int(offsets[-1]) + 1
         out, toff = np.zeros(cap, np.uint32), np.zeros(n + 1, np.uint32)
         self.h.call("smgx_tokenize_batch", self.model, _p(data), _p(offsets), n, _p(out), _p(toff), cap)
         return [out[toff[i]:toff[i + 1]].tolist() for i in range(n)]
@@ -449,6 +450,9 @@ class TiktokenTokenizer:
 
 
 LLAMA3_SPLIT_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|\s+(?!\S)|\s+")
+# Qwen2 / Qwen2.5 / Qwen3 / QwQ: the Llama-3 pattern with \p{N} in place of \p{N}{1,3} (every digit is a piece of its own)
+QWEN2_SPLIT_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|\s+(?!\S)|\s+")
+_SPLIT_PATTERNS = {LLAMA3_SPLIT_PATTERN: _lib.PRETOK_CL100K, QWEN2_SPLIT_PATTERN: _lib.PRETOK_QWEN2}
 
 
 def _byte_level_decoder():
@@ -465,9 +469,9 @@ def _byte_level_decoder():
 
 
 def _hf_pretokenizer(pre):
-    """tokenizer.json `pre_tokenizer` → smgx_pretokenizer, or ValueError for a shape the GPU path does not implement.  Two shapes:
-    Split(Llama-3 / cl100k regex, Isolated) + ByteLevel(use_regex=False), and GPT-2's ByteLevel(use_regex=True, add_prefix_space=False)
-    alone or as a one-element Sequence (its built-in regex is tiktoken's r50k pattern)."""
+    """tokenizer.json `pre_tokenizer` → smgx_pretokenizer, or ValueError for a shape the GPU path does not implement.  Three shapes:
+    Split(Llama-3 / cl100k regex or Qwen2 regex, Isolated) + ByteLevel(use_regex=False), and GPT-2's ByteLevel(use_regex=True,
+    add_prefix_space=False) alone or as a one-element Sequence (its built-in regex is tiktoken's r50k pattern)."""
     steps = pre.get("pretokenizers", [pre]) if pre.get("type") == "Sequence" else [pre]
     kinds = [s.get("type") for s in steps]
     if kinds == ["ByteLevel"]:
@@ -477,17 +481,27 @@ def _hf_pretokenizer(pre):
         raise ValueError("tokenizer.json: a lone ByteLevel pre_tokenizer must have use_regex=True and add_prefix_space=False")
     split = [s for s in steps if s.get("type") == "Split"]
     bl = [s for s in steps if s.get("type") == "ByteLevel"]
-    if kinds != ["Split", "ByteLevel"] or split[0].get("pattern", {}).get("Regex") != LLAMA3_SPLIT_PATTERN or \
+    if kinds != ["Split", "ByteLevel"] or split[0].get("pattern", {}).get("Regex") not in _SPLIT_PATTERNS or \
             str(split[0].get("behavior")).lower() != "isolated" or split[0].get("invert") or bl[0].get("use_regex") or bl[0].get("add_prefix_space"):
-        raise ValueError("tokenizer.json: pre_tokenizer must be Split(Llama-3 regex, Isolated) + ByteLevel(use_regex=False), "
+        raise ValueError("tokenizer.json: pre_tokenizer must be Split(Llama-3 or Qwen2 regex, Isolated) + ByteLevel(use_regex=False), "
                          "or ByteLevel(use_regex=True, add_prefix_space=False) alone")
-    return _lib.PRETOK_CL100K
+    return _SPLIT_PATTERNS[split[0]["pattern"]["Regex"]]
+
+
+def _hf_normalizer(norm):
+    """tokenizer.json `normalizer` → smgx_normalizer: none, or NFC alone or as a one-element Sequence.  Every other normalizer is refused."""
+    if norm is None:
+        return _lib.NORMALIZER_NONE
+    steps = norm.get("normalizers", []) if norm.get("type") == "Sequence" else [norm]
+    if [s.get("type") for s in steps] == ["NFC"]:
+        return _lib.NORMALIZER_NFC
+    raise ValueError("tokenizer.json: the only normalizer supported on the GPU path is NFC (alone or as a one-element Sequence)")
 
 
 class HuggingFaceTokenizer(TiktokenTokenizer):
     """tokenizer::HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs) for the byte-level BPE family the GPU path covers:
-    tokenizer.json with no normalizer, either Split(Llama-3 / cl100k regex, Isolated) + ByteLevel(use_regex=False) or GPT-2's
-    ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk / byte_fallback.  Anything else is
+    tokenizer.json with no normalizer or NFC, either Split(Llama-3 / cl100k or Qwen2 regex, Isolated) + ByteLevel(use_regex=False) or
+    GPT-2's ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk / byte_fallback.  Anything else is
     refused loudly — there is no CPU tokenizer behind this."""
 
     def __init__(self, handle: _Handle, model: str, path: str):   # noqa: D401 — does not call the tiktoken loader
@@ -498,9 +512,11 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         if mdl.get("type") != "BPE" or mdl.get("dropout") or mdl.get("unk_token") or mdl.get("byte_fallback") or \
                 mdl.get("continuing_subword_prefix") or mdl.get("end_of_word_suffix"):
             raise ValueError("tokenizer.json: only plain byte-level BPE models are supported on the GPU path")
-        if j.get("normalizer") is not None:
-            raise ValueError("tokenizer.json: normalizers are not supported on the GPU path")
+        norm = _hf_normalizer(j.get("normalizer"))
         pretok = _hf_pretokenizer(j.get("pre_tokenizer") or {})
+        # NFC goes with the Qwen2 Split or GPT-2's ByteLevel; a Llama-3 Split with a normalizer stays refused, as before
+        if norm != _lib.NORMALIZER_NONE and pretok == _lib.PRETOK_CL100K:
+            raise ValueError("tokenizer.json: a normalizer is supported with the Qwen2 Split or GPT-2's ByteLevel pre_tokenizer, not the Llama-3 Split")
         dec = _byte_level_decoder()
         vocab = mdl["vocab"]
         toks = [bytes(dec[c] for c in s) for s in vocab]
@@ -520,11 +536,16 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         # not, as long as all of them carry the same mark; a mix splits the text in two passes, which the GPU path does not implement.
         if len({bool(a.get("normalized", False)) for a in j.get("added_tokens", [])}) > 1:
             raise ValueError("tokenizer.json: added tokens with mixed `normalized` values are not supported")
+        # With a normalizer, added tokens marked normalized are matched on the normalized text — a second pass the GPU path does not
+        # implement.  Those marked normalized = false are cut from the raw text first, which is what the GPU path does.
+        if norm != _lib.NORMALIZER_NONE and any(a.get("normalized", False) for a in j.get("added_tokens", [])):
+            raise ValueError("tokenizer.json: added tokens with normalized = true are not supported together with a normalizer")
+        self.growth = 3 if norm != _lib.NORMALIZER_NONE else 1   # NFC can grow text threefold
         strs = (C.c_char_p * max(len(added), 1))(*[k.encode() for k, _ in added]) if added else None
         sp_ids = _u32([v for _, v in added])
         mg = _u32(merges)
-        self.h.call("smgx_tokenizer_load_bpe_merges_ex", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
-                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), len(added), pretok)
+        self.h.call("smgx_tokenizer_load_bpe_merges_norm", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
+                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), len(added), pretok, norm)
 
 
 TREE_BATCH_MODES = {"sequential": 0, "snapshot": 1}   # smgx_tree_batch_mode (include/smgx.h)
@@ -539,6 +560,7 @@ class CacheAwarePolicy:
         self.config = config or CacheAwareConfig()
         self._h = _Handle(self.config, device_id, max_batch, max_tokens_per_request, TREE_BATCH_MODES[tree_batch_mode])
         self._slices = {}   # model → tuple(urls) currently registered
+        self._tok_growth = {}   # model → most tokens per byte of text of its tokenizer (3 with a normalizer)
         self._monitor = None
 
     @classmethod
@@ -712,10 +734,14 @@ class CacheAwarePolicy:
 
     # -- tokenizer + text-in pick (the whole hot path on the device) ------------------------------------------------
     def load_tiktoken_tokenizer(self, path: str, special_tokens=None, model: str = UNKNOWN_MODEL_ID, encoding: str = "cl100k_base") -> TiktokenTokenizer:
-        return TiktokenTokenizer(self._h, model, path, special_tokens, encoding)
+        tok = TiktokenTokenizer(self._h, model, path, special_tokens, encoding)
+        self._tok_growth[normalize_model_key(model)] = tok.growth
+        return tok
 
     def load_hf_tokenizer(self, path: str, model: str = UNKNOWN_MODEL_ID) -> HuggingFaceTokenizer:
-        return HuggingFaceTokenizer(self._h, model, path)
+        tok = HuggingFaceTokenizer(self._h, model, path)
+        self._tok_growth[normalize_model_key(model)] = tok.growth
+        return tok
 
     def select_worker_batch_text(self, workers: Sequence[BasicWorker], texts, want_tokens: bool = True):
         """Chat-template-rendered texts → (worker_idx, info, token lists): tokenise on the GPU, then the cache-aware pick,
@@ -725,7 +751,7 @@ class CacheAwarePolicy:
         n = len(texts)
         out = np.full(max(n, 1), -1, dtype=np.int32)
         info = (_lib.DecisionInfo * max(n, 1))()
-        cap = int(offsets[-1]) + 1
+        cap = self._tok_growth.get(model.decode(), 1) * int(offsets[-1]) + 1
         toks, toff = (np.zeros(cap, np.uint32), np.zeros(n + 1, np.uint32)) if want_tokens else (None, None)
         self._h.call("smgx_select_batch_text", model, _p(data), _p(offsets), n, _p(out), C.cast(info, C.c_void_p),
                      _p(toks) if want_tokens else None, _p(toff) if want_tokens else None, cap)
