@@ -492,8 +492,10 @@ void smgx_set_fused_prefetch(int flavour);
 /* Requests per warp of the tiled event kernel (8, 16 or 32; 0 = never use it) and the launch size from which it is used (requests; < 0 =
  * the default, tile × 4 × SM count).  Environment: SMGX_FUSED_TILE. */
 void smgx_set_fused_tile(int tile, int64_t min_total);
-/* The simple event kernel (one warp per request, registers only; default): 0 = off, 4 / 5 / 6 = resident 256-thread CTAs per SM it is compiled
- * for (64 / 48 / 40 registers).  Environment: SMGX_EVENT_SIMPLE. */
+/* The register event kernels (the default for plain picks on fleets of ≤ 64 workers at block size 16): one thread per request
+ * (event_lane_kernel) for launches of at least 256 requests per SM, one warp per request (event_warp_kernel) below that, both with
+ * event_slow_kernel for rare shapes.  0 = off, 4, 5 or 6 = on (the values once chose occupancy variants of the one-warp-per-request
+ * kernel; they are accepted and all mean on).  Environment: SMGX_EVENT_SIMPLE. */
 void smgx_set_event_simple(int min_blocks_per_sm);
 /* Token stream of the tiled kernel: 0 = register double buffer, 4 / 8 = cp.async shared-memory ring of that many requests per warp
  * (SMGX_TILE_DEPTH). */

@@ -19,12 +19,15 @@
 // Contents, in file order:
 //   shared device code     slot probes, worker-set algebra, scan_drain / jump_search (generic search), hash_block
 //   hash_blocks_kernel     the hash stream
-//   event_search_thread_kernel, event_search_warp_kernel, search2_body / event_search2_kernel
-//   alternatives           (SMGX_EVENT_PATH, every one parity-green; on H100 event_simple_kernel below is the default, the pair is `split`)
+//   event_search_thread_kernel, event_search_warp_kernel
+//   finish_pick, drain_resolve   argmax + store of one request; the register drain of a failed count test (search2 and the lane kernel)
+//   search2_body / event_search2_kernel
+//   alternatives           (SMGX_EVENT_PATH, every one parity-green; on H100 event_lane_kernel below is the default, the pair is `split`)
 //       event_hs_kernel        hash stream whose last CTA per 256-request group searches
 //       event_stream_kernel    persistent, warp-specialised, fed by bulk async copies (+ stream_search)
 //       event_tile_kernel      one warp per 8 / 16 / 32 requests
-//       event_simple_kernel    one warp per request in registers, event_slow_kernel for rare shapes
+//       event_lane_kernel      one thread per request, failed count tests drained across the CTA, event_slow_kernel for rare shapes
+//       event_warp_kernel      the same pick, one warp per request, for launches of fewer than 256 requests per SM
 //       event_fused_kernel     persistent warp per request (also the mapped / feedback path)
 //   small kernels          find_matches, content_hashes, fill, fleet_prepare
 //   launchers              path selection (event_path), launch_event_hash / _search / _select
@@ -263,18 +266,39 @@ __device__ __forceinline__ uint4 ld_stream(const uint4* p) {
     asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol));
     return r;
 }
+// the 16 tokens of one block: four evict-first 16 B loads when the block is 16 B aligned, scalar loads otherwise
+__device__ __forceinline__ void load_block16(const uint32_t* __restrict__ p, uint32_t (&w)[16]) {
+    if ((reinterpret_cast<uintptr_t>(p) & 15) == 0) {
+        const uint4* q = reinterpret_cast<const uint4*>(p);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { uint4 t = ld_stream(q + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) w[i] = __ldg(p + i);
+    }
+}
+// two blocks of one request: they lie a multiple of 64 B apart, so one alignment test serves both, and all their loads are issued before
+// either block is hashed (two separate load_block16 branches let the compiler hash the first block before loading the second)
+__device__ __forceinline__ void load_block16_pair(const uint32_t* __restrict__ p0, const uint32_t* __restrict__ p1, uint32_t (&w0)[16], uint32_t (&w1)[16]) {
+    if ((reinterpret_cast<uintptr_t>(p0) & 15) == 0) {
+        const uint4* q0 = reinterpret_cast<const uint4*>(p0);
+        const uint4* q1 = reinterpret_cast<const uint4*>(p1);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint4 t0 = ld_stream(q0 + i), t1 = ld_stream(q1 + i);
+            w0[4 * i] = t0.x; w0[4 * i + 1] = t0.y; w0[4 * i + 2] = t0.z; w0[4 * i + 3] = t0.w;
+            w1[4 * i] = t1.x; w1[4 * i + 1] = t1.y; w1[4 * i + 2] = t1.z; w1[4 * i + 3] = t1.w;
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) { w0[i] = __ldg(p0 + i); w1[i] = __ldg(p1 + i); }
+    }
+}
 template <int BS>
 __device__ __forceinline__ uint64_t hash_block(const uint32_t* __restrict__ p, uint32_t bs) {
     if (BS == 16) {
         uint32_t w[16];
-        if ((reinterpret_cast<uintptr_t>(p) & 15) == 0) {
-            const uint4* q = reinterpret_cast<const uint4*>(p);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { uint4 t = ld_stream(q + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) w[i] = __ldg(p + i);
-        }
+        load_block16(p, w);
         return xxh3_16words(w, kSeed);
     }
     return xxh3_words(p, bs, kSeed);
@@ -601,6 +625,64 @@ __device__ __noinline__ SlowResult fused_slow_search(const EventIndexView* vp, c
     return r;
 }
 
+// argmax + store for one request (any single thread): `win` = eligible workers tied on the best overlap `score` (0: the least-loaded
+// healthy worker); a worker-id-sharded fleet stores this shard's candidate instead of a pick
+__device__ __forceinline__ void finish_pick(const BatchDesc& b, uint32_t r, const int32_t* s_slice, const uint64_t* s_load, const uint64_t* s_ts,
+                                            int32_t min_load_idx, uint64_t win, uint32_t score, uint32_t ntok) {
+    int32_t out = min_load_idx;
+    uint32_t branch = SMGX_BR_EVENT_MIN_LOAD, matched = 0;
+    Cand c{false, 0, 0, -1};
+    if (win) {
+        while (win) { int id = __ffsll((long long)win) - 1; win &= win - 1; c.consider(s_slice[id], s_load[id], s_ts[id]); }
+        out = c.sl; branch = SMGX_BR_EVENT_OVERLAP; matched = score;
+    }
+    if (b.cand) {
+        smgx_shard_candidate sc;
+        sc.score = c.have ? matched : 0; sc.local_idx = c.have ? (uint32_t)c.sl : 0xFFFFFFFFu; sc.load = c.ld; sc.tree_size = c.ts;
+        b.cand[r] = sc;
+    } else write_pick(b, r, out, branch, matched, ntok);
+}
+
+// linear_scan_drain over positions 1..=last (event_tree.rs:582-657) of a request of nb ≤ 32 blocks whose count test failed, from registers:
+// lane p ≤ last holds its probe of position p (found, sl), lane 0's being the Single entry the jump search started from.  The reference's
+// ordered scan with its retain guard is replayed by a ballot loop.  Warp-uniform result: the tied set and its score, or bail = an entry
+// that needs the rolling prefix hash (Multi) was met, and the generic search has to decide.
+struct DrainResult { uint64_t win; uint32_t score; bool bail; };
+__device__ __forceinline__ DrainResult drain_resolve(int nb, uint64_t elig, int lane, bool found, const Slot& sl) {
+    const int last = nb - 1;
+    uint64_t active = shfl64(sl.payload, 0);
+    const bool in_range = lane >= 1 && lane <= last;
+    const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
+    uint64_t last_set = 0;
+    uint32_t last_score = 0;
+    bool bail = !__shfl_sync(FULL, (int)found, 0) || __shfl_sync(FULL, sl.state, 0) != SLOT_SINGLE;
+    unsigned remaining = __ballot_sync(FULL, in_range);
+    while (!bail && remaining && active) {
+        const uint32_t nact = (uint32_t)__popcll(active);
+        const bool noop = found && sl.state == SLOT_SINGLE && cnt >= nact;           // retain guard (:611, :641)
+        const unsigned bm = __ballot_sync(FULL, in_range && !noop) & remaining;
+        if (!bm) break;
+        const int k = __ffs((int)bm) - 1;
+        if (!__shfl_sync(FULL, (int)found, k)) {                                     // missing entry drains everything (:598-604)
+            const uint64_t e = active & elig;
+            if (e) { last_set = e; last_score = (uint32_t)k; }
+            active = 0;
+            break;
+        }
+        if (__shfl_sync(FULL, sl.state, k) != SLOT_SINGLE) { bail = true; break; }
+        const uint64_t ws = shfl64(sl.payload, k);
+        if ((uint32_t)__popcll(ws) < nact) {
+            const uint64_t e = active & ~ws & elig;
+            if (e) { last_set = e; last_score = (uint32_t)k; }
+            active &= ws;
+        }
+        remaining &= ~((2u << k) - 1u);
+    }
+    DrainResult d{active & elig, (uint32_t)nb, bail};
+    if (!d.win) { d.win = last_set; d.score = last_score; }
+    return d;
+}
+
 // ---- search + pick, fleets of ≤ 64 interned workers, second version: balanced drains -------------------------------------------
 // event_search_thread_kernel above is one partial wave whose duration is set by its UNLUCKIEST warp: every request whose count test
 // fails (a stored prefix shorter than the request: ≈ 10 % of BASELINE config 2) is drained in its home warp, one after another, two to
@@ -675,19 +757,8 @@ __device__ __forceinline__ void search2_body(const EventIndexView& v, const Flee
     const bool cand_mode = b.cand != nullptr;
     const FleetDerived fd = *f.derived;
     const uint64_t elig = f.elig[0];
-    auto finish = [&](uint32_t r, uint64_t win, uint32_t score, uint32_t ntok) {   // argmax + store for one request (any single thread)
-        int32_t out = fd.min_load_idx;
-        uint32_t branch = SMGX_BR_EVENT_MIN_LOAD, matched = 0;
-        Cand c{false, 0, 0, -1};
-        if (win) {
-            while (win) { int id = __ffsll((long long)win) - 1; win &= win - 1; c.consider(s_slice[id], s_load[id], s_ts[id]); }
-            out = c.sl; branch = SMGX_BR_EVENT_OVERLAP; matched = score;
-        }
-        if (cand_mode) {
-            smgx_shard_candidate sc;
-            sc.score = c.have ? matched : 0; sc.local_idx = c.have ? (uint32_t)c.sl : 0xFFFFFFFFu; sc.load = c.ld; sc.tree_size = c.ts;
-            b.cand[r] = sc;
-        } else write_pick(b, r, out, branch, matched, ntok);
+    auto finish = [&](uint32_t r, uint64_t win, uint32_t score, uint32_t ntok) {
+        finish_pick(b, r, s_slice, s_load, s_ts, fd.min_load_idx, win, score, ntok);
     };
 
     // ---- phase A ----
@@ -726,42 +797,10 @@ __device__ __forceinline__ void search2_body(const EventIndexView& v, const Flee
     //      hash loads and the probes of the second overlap those of the first ----
     const uint32_t n_b = s_nb;
     auto resolve = [&](const Search2Item it, bool found, const Slot& sl) {
-        const int last = (int)it.nb - 1;
-        uint64_t active = shfl64(sl.payload, 0);                                        // phase A saw a Single entry at position 0
-        const bool in_range = lane >= 1 && lane <= last;
-        const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
-        uint64_t last_set = 0;
-        uint32_t last_score = 0;
-        bool bail = !__shfl_sync(FULL, (int)found, 0) || __shfl_sync(FULL, sl.state, 0) != SLOT_SINGLE;
-        unsigned remaining = __ballot_sync(FULL, in_range);
-        while (!bail && remaining && active) {
-            const uint32_t nact = (uint32_t)__popcll(active);
-            const bool noop = found && sl.state == SLOT_SINGLE && cnt >= nact;           // retain guard (:611, :641)
-            const unsigned bm = __ballot_sync(FULL, in_range && !noop) & remaining;
-            if (!bm) break;
-            const int k = __ffs((int)bm) - 1;
-            if (!__shfl_sync(FULL, (int)found, k)) {                                     // missing entry drains everything (:598-604)
-                const uint64_t e = active & elig;
-                if (e) { last_set = e; last_score = (uint32_t)k; }
-                active = 0;
-                break;
-            }
-            if (__shfl_sync(FULL, sl.state, k) != SLOT_SINGLE) { bail = true; break; }
-            const uint64_t ws = shfl64(sl.payload, k);
-            if ((uint32_t)__popcll(ws) < nact) {
-                const uint64_t e = active & ~ws & elig;
-                if (e) { last_set = e; last_score = (uint32_t)k; }
-                active &= ws;
-            }
-            remaining &= ~((2u << k) - 1u);
-        }
-        if (bail) { if (lane == 0) { const uint32_t qq = atomicAdd(&s_nc, 1u); s_qc[qq] = it; } }
-        else if (lane == 0) {
-            uint64_t win = active & elig;
-            uint32_t score = it.nb;
-            if (!win) { win = last_set; score = last_score; }
-            finish(it.r, win, score, b.out_info ? ld_rec((uint64_t)b.hash_base + it.r).ntok : 0u);   // ntok only feeds out_info: no round trip without it
-        }
+        const DrainResult d = drain_resolve((int)it.nb, elig, lane, found, sl);
+        if (lane != 0) return;
+        if (d.bail) { const uint32_t qq = atomicAdd(&s_nc, 1u); s_qc[qq] = it; }
+        else finish(it.r, d.win, d.score, b.out_info ? ld_rec((uint64_t)b.hash_base + it.r).ntok : 0u);   // ntok only feeds out_info: no round trip without it
     };
     constexpr uint32_t NW = NT / 32;
     for (uint32_t q = wic; q < n_b; q += 2 * NW) {
@@ -1492,16 +1531,19 @@ __global__ void __launch_bounds__(128, MINB) event_tile_kernel(const __grid_cons
     }
 }
 
-// ---- the same pick, SIMPLE: one warp per request, no persistence, no software pipeline ------------------------------------------
-// What the measurements of the two kernels above say: a warp that walks several requests pays each request's DRAM latency in sequence
-// (tile kernel: 183 instructions per request but few warps per SM doing anything), and software pipelining costs registers and
-// bookkeeping instructions (440 per request, issue-bound).  The cheapest way to keep ≥ 64 KB per SM in flight is the hardware's own
-// warp scheduler: ONE request per warp, as many warps per SM as the register budget allows, a grid of ⌈requests / 8⌉ CTAs that the block
-// scheduler streams through the SMs.  Everything lives in registers: lane p owns block p.  Lanes 0 and last hash their blocks and probe
-// the two jump destinations; only a failed count test makes lanes 1..last-1 read and hash theirs, and then positions 1..last are drained
-// with one parallel probe per lane and an ordered ballot loop (linear_scan_drain with the retain guard, event_tree.rs:582-657).  A full
-// hit or a novel request thus reads 128 B of tokens, not all of them.  Only what needs the rolling prefix hashes or more than one jump
-// (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device queue and finished by event_slow_kernel right behind.
+// ---- the same pick, ONE THREAD per request, rare shapes queued for event_slow_kernel --------------------------------------------
+// One warp per request (event_warp_kernel below) keeps 40 requests in flight per SM, and a full hit runs the whole warp's instruction
+// stream for two useful lanes: that pick is bound by latency and instruction issue, not by bytes.  Here a CTA of 256 threads decides 256
+// consecutive requests g (global index over the launch's batches: a CTA may straddle two batches) in two phases:
+//   A  one THREAD per request: offsets, the fleet gate, the tokens of blocks 0 and last (all eight 16 B loads issued before either hash),
+//      both hashes, both probes in flight together, the count-only jump test (event_tree.rs:720).  A block's content hash depends on
+//      that block alone, so a full hit or a novel request reads 128 B of tokens.  A failed count test goes onto a shared-memory queue
+//      together with both hashes;
+//   B  the queue is striped over the CTA's 8 warps, two drains per round so that the loads and probes of the second overlap those of
+//      the first: lane p (1 ≤ p < last) reads and hashes block p, lanes 0 and last take the queued hashes, every position is probed at
+//      once and drain_resolve replays the ordered scan.
+// What needs the rolling prefix hashes or more than one jump (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device
+// queue, at most once per request (from A or from B), and finished by event_slow_kernel right behind.
 struct SimpleLoc { uint32_t j, r; };
 __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t g) {
     SimpleLoc l;
@@ -1510,9 +1552,102 @@ __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t 
     return l;
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
-                                                                  uint32_t* __restrict__ slow_queue) {
+struct LaneDrain { uint32_t g, off, ntok, pad; uint64_t c0, c1; };   // a failed count test: request, token range, hashes of blocks 0 and last
+
+__global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
+                                                            uint32_t* __restrict__ slow_queue) {
+    __shared__ int32_t s_slice[64];
+    __shared__ uint64_t s_load[64], s_ts[64];
+    __shared__ LaneDrain s_q[256];
+    __shared__ uint32_t s_n;
+    if (threadIdx.x < 64) {
+        bool ok = threadIdx.x < v.n_workers;
+        s_slice[threadIdx.x] = ok ? f.slice_of_id[threadIdx.x] : -1;
+        s_load[threadIdx.x] = ok ? f.load_of_id[threadIdx.x] : 0;
+        s_ts[threadIdx.x] = ok ? v.tree_sizes[threadIdx.x] : 0;
+    }
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    const int32_t min_load_idx = f.derived->min_load_idx;
+    const uint64_t elig = f.elig[0];
+    auto to_slow = [&](uint32_t g) { slow_queue[2 + atomicAdd(slow_queue, 1u)] = g; };
+
+    // ---- phase A ----
+    const uint32_t g = blockIdx.x * 256 + threadIdx.x;
+    if (g < a.total) {
+        const SimpleLoc loc = simple_locate(a, g);
+        const BatchDesc& b = a.b[loc.j];
+        const uint32_t off = __ldg(b.offsets + loc.r), ntok = __ldg(b.offsets + loc.r + 1) - off;
+        const uint32_t nb = ntok >> 4;
+        if (f.derived->n_healthy == 0) write_pick(b, loc.r, -1, SMGX_BR_NO_HEALTHY, 0, ntok);
+        else if (f.derived->imbalanced) write_pick(b, loc.r, min_load_idx, SMGX_BR_IMBALANCED_MIN_LOAD, 0, ntok);
+        else if (nb > a.max_blocks) { atomicExch(a.err_flag, 1u); write_pick(b, loc.r, -1, 255, 0, ntok); }
+        else if (nb == 0 || v.n_workers == 0) finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, 0, 0, ntok);
+        else if (nb > 32 || nb - 1 > v.jump) to_slow(g);   // more than one jump / more blocks than lanes: the generic search
+        else {
+            const uint32_t last = nb - 1;
+            uint32_t w0[16], w1[16];
+            load_block16_pair(b.tokens + off, b.tokens + off + (size_t)last * 16, w0, w1);
+            const uint64_t c0 = xxh3_16words(w0, kSeed), c1 = xxh3_16words(w1, kSeed);
+            const uint32_t h0 = slot_hash(0, c0) & v.mask, h1 = slot_hash(last, c1) & v.mask;
+            Slot s0 = load_slot(v.slots + h0), s1 = load_slot(v.slots + h1);   // both probes in flight together
+            if (!finish_probe(v, 0, c0, h0, s0)) finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, 0, 0, ntok);   // nothing cached at 0 (:676-683)
+            else if (s0.state != SLOT_SINGLE) to_slow(g);
+            else if (s0.payload == 0 || last == 0) finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, s0.payload & elig, nb, ntok);
+            else {
+                const bool f1 = finish_probe(v, last, c1, h1, s1);
+                if (f1 && s1.state != SLOT_SINGLE) to_slow(g);
+                else if (f1 && __popcll(s1.payload) == __popcll(s0.payload))   // count-only jump test (:720)
+                    finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, s0.payload & elig, nb, ntok);
+                else s_q[atomicAdd(&s_n, 1u)] = LaneDrain{g, off, ntok, 0, c0, c1};
+            }
+        }
+    }
+    __syncthreads();
+
+    // ---- phase B: one warp per queued drain, the queue striped over the 8 warps, two drains per round ----
+    const int lane = threadIdx.x & 31;
+    const uint32_t n_d = s_n;
+    auto drain_done = [&](const LaneDrain& d, const DrainResult& r) {   // lane 0
+        if (r.bail) { to_slow(d.g); return; }
+        const SimpleLoc l = simple_locate(a, d.g);
+        finish_pick(a.b[l.j], l.r, s_slice, s_load, s_ts, min_load_idx, r.win, r.score, d.ntok);
+    };
+    for (uint32_t q = threadIdx.x >> 5; q < n_d; q += 16) {
+        const bool two = q + 8 < n_d;
+        const LaneDrain& d0 = s_q[q];
+        const LaneDrain& d1 = s_q[two ? q + 8 : q];
+        const int last0 = (int)(d0.ntok >> 4) - 1, last1 = two ? (int)(d1.ntok >> 4) - 1 : -1;   // last1 = -1: no second drain this round
+        const bool m0 = lane >= 1 && lane < last0, m1 = lane >= 1 && lane < last1;
+        uint32_t w0[16], w1[16];
+        if (m0) load_block16(a.b[simple_locate(a, d0.g).j].tokens + d0.off + (size_t)lane * 16, w0);
+        if (m1) load_block16(a.b[simple_locate(a, d1.g).j].tokens + d1.off + (size_t)lane * 16, w1);
+        uint64_t h0 = lane == 0 ? d0.c0 : d0.c1, h1 = lane == 0 ? d1.c0 : d1.c1;
+        if (m0) h0 = xxh3_16words(w0, kSeed);
+        if (m1) h1 = xxh3_16words(w1, kSeed);
+        // every position of both requests probed at once (0 and last again: L2-hot)
+        const uint32_t i0 = slot_hash((uint32_t)lane, h0) & v.mask, i1 = slot_hash((uint32_t)lane, h1) & v.mask;
+        Slot sl0{0, 0, SLOT_EMPTY, 0, 0}, sl1{0, 0, SLOT_EMPTY, 0, 0};
+        if (lane <= last0) sl0 = load_slot(v.slots + i0);
+        if (lane <= last1) sl1 = load_slot(v.slots + i1);
+        bool f0 = false, f1 = false;
+        if (lane <= last0) f0 = finish_probe(v, (uint32_t)lane, h0, i0, sl0);
+        if (lane <= last1) f1 = finish_probe(v, (uint32_t)lane, h1, i1, sl1);
+        const DrainResult r0 = drain_resolve(last0 + 1, elig, lane, f0, sl0);
+        if (lane == 0) drain_done(d0, r0);
+        if (two) {
+            const DrainResult r1 = drain_resolve(last1 + 1, elig, lane, f1, sl1);
+            if (lane == 0) drain_done(d1, r1);
+        }
+    }
+}
+
+// The same pick with one WARP per request, for launches too small to give every SM a CTA of event_lane_kernel (a lone batch of a few
+// thousand requests): ⌈requests / 8⌉ CTAs spread the work over all SMs, where the lane kernel's ⌈requests / 256⌉ would occupy a few.
+// Lane p owns block p; lanes 0 and last hash their blocks and probe the two jump destinations, and only a failed count test makes lanes
+// 1..last-1 read and hash theirs for drain_resolve.  Rare shapes go to the same queue for event_slow_kernel.
+__global__ void __launch_bounds__(256, 5) event_warp_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
+                                                            uint32_t* __restrict__ slow_queue) {
     __shared__ int32_t s_slice[64];
     __shared__ uint64_t s_load[64], s_ts[64];
     if (threadIdx.x < 64) {
@@ -1544,8 +1679,6 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
                     return;
                 }
                 const int last = (int)nb - 1;
-                // a block's content hash depends on that block alone, so only the two positions the jump search probes are hashed
-                // up front; the blocks in between are read only if the count test fails and the drain needs them
                 Slot sl{0, 0, SLOT_EMPTY, 0, 0};
                 bool found = false;
                 if (lane == 0 || lane == last) found = probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
@@ -1556,45 +1689,19 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
                 if (__shfl_sync(FULL, (int)found, 0)) {
                     if (__shfl_sync(FULL, sl.state, 0) != SLOT_SINGLE) bail = true;   // Multi at position 0: needs the prefix hash
                     else {
-                        uint64_t active = shfl64(sl.payload, 0);
+                        const uint64_t active = shfl64(sl.payload, 0);
+                        win = active & elig; score = nb;
                         if (last > 0 && active) {
                             const bool fl = __shfl_sync(FULL, (int)found, last) != 0;
                             const uint32_t stl = __shfl_sync(FULL, sl.state, last);
                             uint32_t count = 0;   // count_workers_at(last) (:555-574)
                             if (fl) { if (stl == SLOT_SINGLE) count = (uint32_t)__popcll(shfl64(sl.payload, last)); else bail = true; }
                             if (!bail && count != (uint32_t)__popcll(active)) {
-                                // linear_scan_drain over positions 1..=last (:582-657): every position probed at once, one lane each
-                                const bool in_range = lane >= 1 && lane <= last;
                                 if (lane >= 1 && lane < last) found = probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
-                                const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
-                                uint64_t last_set = 0;
-                                uint32_t last_score = 0;
-                                unsigned remaining = __ballot_sync(FULL, in_range);
-                                while (remaining && active) {
-                                    const uint32_t nact = (uint32_t)__popcll(active);
-                                    const bool noop = found && sl.state == SLOT_SINGLE && cnt >= nact;   // retain guard (:611, :641)
-                                    const unsigned bm = __ballot_sync(FULL, in_range && !noop) & remaining;
-                                    if (!bm) break;
-                                    const int k = __ffs((int)bm) - 1;
-                                    if (!__shfl_sync(FULL, (int)found, k)) {   // missing entry drains everything (:598-604)
-                                        const uint64_t e = active & elig;
-                                        if (e) { last_set = e; last_score = (uint32_t)k; }
-                                        active = 0;
-                                        break;
-                                    }
-                                    if (__shfl_sync(FULL, sl.state, k) != SLOT_SINGLE) { bail = true; break; }
-                                    const uint64_t ws = shfl64(sl.payload, k);
-                                    if ((uint32_t)__popcll(ws) < nact) {
-                                        const uint64_t e = active & ~ws & elig;
-                                        if (e) { last_set = e; last_score = (uint32_t)k; }
-                                        active &= ws;
-                                    }
-                                    remaining &= ~((2u << k) - 1u);
-                                }
-                                win = active & elig; score = nb;
-                                if (!win) { win = last_set; score = last_score; }
-                            } else { win = active & elig; score = nb; }
-                        } else { win = active & elig; score = nb; }
+                                const DrainResult d = drain_resolve((int)nb, elig, lane, found, sl);
+                                bail = d.bail; win = d.win; score = d.score;
+                            }
+                        }
                     }
                 }
                 if (bail) {
@@ -1612,7 +1719,7 @@ __global__ void __launch_bounds__(256, MINB) event_simple_kernel(const __grid_co
     if (lane == 0) write_pick(b, loc.r, out, branch, matched, ntok);
 }
 
-// the queue of event_simple_kernel: generic warp-cooperative search, one warp per queued request (hashes staged in a shared-memory row)
+// the queue of event_lane_kernel / event_warp_kernel: generic warp-cooperative search, one warp per queued request (hashes staged in a shared-memory row)
 __global__ void __launch_bounds__(256) event_slow_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
                                                          uint32_t* __restrict__ slow_queue) {
     extern __shared__ uint64_t smem_ch[];
@@ -1997,7 +2104,7 @@ static int fused_tile() {   // SMGX_FUSED_TILE=0|8|16|32: requests per warp of t
 }
 static std::atomic<int> g_simple{-1};
 void set_event_simple(int minb) { g_simple.store(minb, std::memory_order_relaxed); }
-static int event_simple_minb() {   // SMGX_EVENT_SIMPLE=0|4|5|6: resident CTAs per SM the simple kernel is compiled for (0 = do not use it)
+static bool event_lane_selected() {   // SMGX_EVENT_SIMPLE=0|4|5|6: 0 = do not use the lane / warp kernels, 4 / 5 / 6 = use them (the default)
     int v = g_simple.load(std::memory_order_relaxed);
     if (v < 0) {
         const char* e = getenv("SMGX_EVENT_SIMPLE");
@@ -2005,17 +2112,19 @@ static int event_simple_minb() {   // SMGX_EVENT_SIMPLE=0|4|5|6: resident CTAs p
         if (v != 0 && v != 4 && v != 5 && v != 6) v = 5;
         g_simple.store(v, std::memory_order_relaxed);
     }
-    return v;
+    return v != 0;
 }
-static void launch_simple(const EventIndexView& ix, const FleetView& fleet, const MultiArgs& a, int sm_count, cudaStream_t stream, uint32_t* d_queue, int minb) {
-    const unsigned grid = (a.total + 7) / 8;
-    if (minb == 4) event_simple_kernel<4><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
-    else if (minb == 6) event_simple_kernel<6><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
-    else event_simple_kernel<5><<<grid, 256, 0, stream>>>(ix, fleet, a, d_queue);
+static void launch_lane(const EventIndexView& ix, const FleetView& fleet, const MultiArgs& a, int sm_count, cudaStream_t stream, uint32_t* d_queue) {
+    // one thread per request once the launch gives every SM a CTA of 256; below that (a lone batch of a few thousand requests) one warp per
+    // request spreads the work over all SMs and answers sooner (measured on H100: 4096 requests, §5 of DESIGN.md)
+    if (a.total >= 256u * (unsigned)sm_count) event_lane_kernel<<<(a.total + 255) / 256, 256, 0, stream>>>(ix, fleet, a, d_queue);
+    else event_warp_kernel<<<(a.total + 7) / 8, 256, 0, stream>>>(ix, fleet, a, d_queue);
     SMGX_CUDA(cudaGetLastError());
     const size_t smem = (size_t)std::max<uint32_t>(a.max_blocks, 1) * 8 * 8;
     if (smem > 48 * 1024) SMGX_CUDA(cudaFuncSetAttribute(event_slow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    event_slow_kernel<<<std::min<unsigned>((unsigned)sm_count * 2, std::max(1u, grid)), 256, smem, stream>>>(ix, fleet, a, d_queue);
+    // one warp per queued request: ⌈total / 8⌉ CTAs would give every request a warp, two per SM are plenty for the rare shapes it gets
+    const unsigned slow_grid = std::min<unsigned>((unsigned)sm_count * 2, std::max(1u, (a.total + 7) / 8));
+    event_slow_kernel<<<slow_grid, 256, smem, stream>>>(ix, fleet, a, d_queue);
     SMGX_CUDA(cudaGetLastError());
 }
 
@@ -2191,13 +2300,12 @@ void launch_event_select(const EventIndexView& ix, const FleetView& fleet, const
     }
     {
         const bool w1 = ix.words == 1;
-        const int simple = needs_fused_kernel(a) ? 0 : event_simple_minb();
-        // the simple kernel: one warp per request, everything in registers, rare shapes queued for event_slow_kernel (see event_simple_kernel)
-        if (simple && w1 && a.block_size == 16 && a.slow_queue && a.max_blocks * 8 * 8 <= 200 * 1024) {
+        // one thread per request, rare shapes queued for event_slow_kernel (see event_lane_kernel)
+        if (!needs_fused_kernel(a) && event_lane_selected() && w1 && a.block_size == 16 && a.slow_queue && a.max_blocks * 8 * 8 <= 200 * 1024) {
             bool plain = true;
             for (uint32_t j = 0; j < a.count; ++j) plain = plain && a.b[j].cand == nullptr;
             if (plain) {
-                launch_simple(ix, fleet, a, sm_count, stream, a.slow_queue, simple);
+                launch_lane(ix, fleet, a, sm_count, stream, a.slow_queue);
                 *launches += 2;
                 return;
             }

@@ -85,7 +85,7 @@ struct MultiArgs {
     uint32_t ready_target[kMaxMultiBatches];
     const void* pf_slots;          // EventIndexView.slots (nullable)
     uint32_t pf_mask, pf_jump;
-    uint32_t* slow_queue;          // event_simple_kernel → event_slow_kernel: [0] = count, [1] = CTA exit counter (both zero between launches), [2 .. total + 1] = request indices
+    uint32_t* slow_queue;          // event_lane_kernel / event_warp_kernel → event_slow_kernel: [0] = count, [1] = CTA exit counter (both zero between launches), [2 .. total + 1] = request indices (each request pushed at most once)
     uint64_t* fb_winsets;
     uint32_t* fb_scores;           // 0xFFFFFFFF = request longer than max_blocks
     // one-launch path (event_hs_kernel): per (batch, group of 256 requests) arrival counters, zero between launches

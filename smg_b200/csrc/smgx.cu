@@ -81,7 +81,7 @@ struct Lane {
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr, t0 = nullptr, t1 = nullptr;
     DevBuf d_fb;   // load-feedback scratch: per-request tied sets + scores
-    DevBuf d_slowq;   // queue between event_simple_kernel and event_slow_kernel
+    DevBuf d_slowq;   // queue between event_lane_kernel / event_warp_kernel and event_slow_kernel
     DevBuf d_recs;    // SearchRec per request: hash kernel → search kernel
     DevBuf d_groups;  // event_hs_kernel's arrival counters, [kMaxMultiBatches][group_stride] (zeroed once; self-resetting)
     uint32_t group_stride = 0;
