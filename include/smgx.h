@@ -377,10 +377,31 @@ smgx_status smgx_tokenizer_load_bpe_merges_norm(smgx_policy* p, const char* mode
                                                 uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, int ignore_merges,
                                                 const char* const* special_strs, const uint32_t* special_ids, uint32_t n_special,
                                                 smgx_pretokenizer pretokenizer, smgx_normalizer normalizer, char** err);
+/* SentencePiece-style BPE tokenizer.json files (Llama 2, CodeLlama, Mistral, Mixtral, TinyLlama): model.type = "BPE" with
+ * byte_fallback = true, the 256 tokens "<0x00>" … "<0xFF>" and "▁" (U+2581) in the vocabulary, no dropout / continuing_subword_prefix /
+ * end_of_word_suffix, ignore_merges = false.  Spaces become ▁ and a stretch of text between added tokens starts with ▁, in one of two shapes:
+ *   SMGX_SP_LEGACY     normalizer Sequence[Prepend("▁"), Replace(" " → "▁")], pre_tokenizer null: every non-empty stretch gets a ▁ in
+ *                      front; prepend_scheme must be SMGX_PREPEND_ALWAYS and split 0;
+ *   SMGX_SP_METASPACE  normalizer null, pre_tokenizer Metaspace(replacement "▁", prepend_scheme, split): a ▁ is prepended unless the
+ *                      stretch already starts with one — SMGX_PREPEND_FIRST only to the stretch at offset 0 of the text, SMGX_PREPEND_NEVER
+ *                      never; split = 1 cuts the stretch before every ▁.
+ * Tokens are RAW UTF-8 strings (no byte-level mapping), merges and specials as for smgx_tokenizer_load_bpe_merges_ex; added tokens are
+ * matched on the raw text.  Initial symbols are code points; one that is not in the vocabulary becomes the <0xXX> tokens of its bytes.
+ * Without split, the GPU merges the pieces of a stretch cut before every ▁ that follows another character; the load refuses
+ * (SMGX_TOKENIZATION_ERROR, naming the merge) a vocabulary with a merge (a, b) where `a` does not end in ▁ and `b` starts with ▁, the one
+ * case where that cut would change the result.  A missing ▁ or byte token is SMGX_TOKENIZATION_ERROR; an unknown enum value, split other
+ * than 0 / 1 or a null pointer is SMGX_INVALID_ARGUMENT. */
+typedef enum smgx_sp_shape { SMGX_SP_LEGACY = 0, SMGX_SP_METASPACE = 1 } smgx_sp_shape;
+typedef enum smgx_prepend_scheme { SMGX_PREPEND_NEVER = 0, SMGX_PREPEND_FIRST = 1, SMGX_PREPEND_ALWAYS = 2 } smgx_prepend_scheme;
+smgx_status smgx_tokenizer_load_bpe_metaspace(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                              uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, const char* const* special_strs,
+                                              const uint32_t* special_ids, uint32_t n_special, smgx_sp_shape shape, smgx_prepend_scheme prepend_scheme,
+                                              int split, char** err);
 /* Encoder::encode_batch (tiktoken.rs:464-469) on the GPU: text i = text[offsets[i] .. offsets[i+1]) (UTF-8, already
  * chat-template-rendered; special-token strings are recognised, tiktoken.rs:446-460).  Writes the ragged token ids and
  * out_tok_offsets[n+1]; `cap_tokens` = capacity of out_tokens: total text bytes is always enough for a tokenizer without a
- * normalizer, 3 × total text bytes for a normalizing one (NFC can grow text threefold, e.g. U+1D160 → three code points). */
+ * normalizer, 3 × total text bytes for a normalizing one (NFC can grow text threefold, e.g. U+1D160 → three code points), and
+ * 2 × total text bytes for a SentencePiece-style one (a stretch of L bytes has at most L + 1 initial symbols: the prepended ▁). */
 smgx_status smgx_tokenize_batch(smgx_policy* p, const char* model_key, const uint8_t* text, const uint32_t* offsets, uint32_t n,
                                 uint32_t* out_tokens, uint32_t* out_tok_offsets, uint32_t cap_tokens, char** err);
 /* The whole hot path in one call: tokenize on the device → cache-aware pick; the token ids never visit the host unless

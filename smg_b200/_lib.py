@@ -12,6 +12,8 @@ SUCCESS, INVALID_ARGUMENT, TOKENIZATION_ERROR, MEMORY_ERROR, DEVICE_ERROR = 0, 1
 WORKER_NOT_TRACKED, PARENT_BLOCK_NOT_FOUND, NOT_FOUND, BUSY, UNKNOWN_ERROR = 10, 11, 12, 13, 99
 PRETOK_CL100K, PRETOK_R50K, PRETOK_QWEN2 = 0, 1, 2   # smgx_pretokenizer
 NORMALIZER_NONE, NORMALIZER_NFC = 0, 1   # smgx_normalizer
+SP_LEGACY, SP_METASPACE = 0, 1   # smgx_sp_shape
+PREPEND_NEVER, PREPEND_FIRST, PREPEND_ALWAYS = 0, 1, 2   # smgx_prepend_scheme
 
 BRANCHES = ["no_healthy", "imbalanced_min_load", "event_overlap", "event_min_load", "tree_match", "tree_min_load",
             "tree_fallback_first_healthy", "no_tree_random"]
@@ -145,6 +147,7 @@ def load():
     sig("smgx_tokenizer_load_tiktoken_ex", st, vp, cp, vp, vp, vp, u32, P(cp), vp, u32, C.c_int, pp)
     sig("smgx_tokenizer_load_bpe_merges_ex", st, vp, cp, vp, vp, vp, u32, vp, u32, C.c_int, P(cp), vp, u32, C.c_int, pp)
     sig("smgx_tokenizer_load_bpe_merges_norm", st, vp, cp, vp, vp, vp, u32, vp, u32, C.c_int, P(cp), vp, u32, C.c_int, C.c_int, pp)
+    sig("smgx_tokenizer_load_bpe_metaspace", st, vp, cp, vp, vp, vp, u32, vp, u32, P(cp), vp, u32, C.c_int, C.c_int, C.c_int, pp)
     sig("smgx_tokenize_batch", st, vp, cp, vp, vp, u32, vp, vp, u32, pp)
     sig("smgx_select_batch_text", st, vp, cp, vp, vp, u32, vp, vp, vp, vp, u32, pp)
     sig("smgx_select_batch_tokens", st, vp, cp, vp, vp, u32, vp, vp, pp)

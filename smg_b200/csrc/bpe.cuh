@@ -319,10 +319,8 @@ SMGX_HD bool piece_lookup(const BpeView& v, const uint8_t* p, uint32_t n, uint32
     }
 }
 
-// tiktoken `_byte_pair_merge` over token ids: ids[0..n) start as the single-byte tokens of the piece, rk[i] packs
-// (rank, merged id) of the pair (ids[i], ids[i+1]).  Returns the number of tokens left in ids[].
-SMGX_HD uint32_t byte_pair_merge(const BpeView& v, const uint8_t* p, uint32_t n, uint32_t* ids, uint64_t* rk) {
-    for (uint32_t i = 0; i < n; ++i) ids[i] = v.byte_token[p[i]];
+// The merge loop of byte_pair_merge on symbols already in ids[0..n) (SentencePiece-style BPE: code points and byte-fallback tokens).
+SMGX_HD uint32_t merge_symbols(const BpeView& v, uint32_t* ids, uint32_t n, uint64_t* rk) {
     if (n < 2) return n;
     for (uint32_t i = 0; i + 1 < n; ++i) rk[i] = pair_lookup(v, ids[i], ids[i + 1]);
     uint32_t m = n;
@@ -340,6 +338,12 @@ SMGX_HD uint32_t byte_pair_merge(const BpeView& v, const uint8_t* p, uint32_t n,
         if (bi > 0) rk[bi - 1] = pair_lookup(v, ids[bi - 1], ids[bi]);
     }
     return m;
+}
+// tiktoken `_byte_pair_merge` over token ids: ids[0..n) start as the single-byte tokens of the piece, rk[i] packs
+// (rank, merged id) of the pair (ids[i], ids[i+1]).  Returns the number of tokens left in ids[].
+SMGX_HD uint32_t byte_pair_merge(const BpeView& v, const uint8_t* p, uint32_t n, uint32_t* ids, uint64_t* rk) {
+    for (uint32_t i = 0; i < n; ++i) ids[i] = v.byte_token[p[i]];
+    return merge_symbols(v, ids, n, rk);
 }
 
 // Longest special token starting at s[i], if any (special strings are matched before the regex, tiktoken `encode`).

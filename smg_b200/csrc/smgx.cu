@@ -1709,6 +1709,36 @@ smgx_status smgx_tokenizer_load_bpe_merges_norm(smgx_policy* p, const char* mode
         return SMGX_SUCCESS;
     });
 }
+smgx_status smgx_tokenizer_load_bpe_metaspace(smgx_policy* p, const char* model_key, const uint8_t* blob, const uint32_t* tok_offsets, const uint32_t* ids,
+                                              uint32_t n_tokens, const uint32_t* merges, uint32_t n_merges, const char* const* special_strs,
+                                              const uint32_t* special_ids, uint32_t n_special, smgx_sp_shape shape, smgx_prepend_scheme prepend_scheme,
+                                              int split, char** err) {
+    return guard(err, [&]() {
+        NONNULL(p); NONNULL(blob); NONNULL(tok_offsets); NONNULL(ids);
+        SMGX_REQUIRE(n_merges == 0 || merges, "Invalid arguments: null pointer");
+        SMGX_REQUIRE(shape == SMGX_SP_LEGACY || shape == SMGX_SP_METASPACE, "Invalid arguments: unknown shape " + std::to_string((int)shape));
+        SMGX_REQUIRE(prepend_scheme == SMGX_PREPEND_NEVER || prepend_scheme == SMGX_PREPEND_FIRST || prepend_scheme == SMGX_PREPEND_ALWAYS,
+                     "Invalid arguments: unknown prepend_scheme " + std::to_string((int)prepend_scheme));
+        SMGX_REQUIRE(split == 0 || split == 1, "Invalid arguments: split must be 0 or 1, not " + std::to_string(split));
+        SMGX_REQUIRE(shape == SMGX_SP_METASPACE || (prepend_scheme == SMGX_PREPEND_ALWAYS && split == 0),
+                     "Invalid arguments: the legacy shape takes prepend_scheme SMGX_PREPEND_ALWAYS and split 0");
+        MetaspaceMode ms{1, shape == SMGX_SP_LEGACY ? (uint32_t)MS_PREPEND_LEGACY
+                            : prepend_scheme == SMGX_PREPEND_NEVER ? (uint32_t)MS_PREPEND_NEVER
+                            : prepend_scheme == SMGX_PREPEND_FIRST ? (uint32_t)MS_PREPEND_FIRST : (uint32_t)MS_PREPEND_ALWAYS,
+                         (uint32_t)split};
+        std::lock_guard<std::mutex> g(p->impl.mu);
+        bool dev = p->impl.cfg.device_id >= 0;
+        if (dev) p->impl.use_device();
+        std::vector<std::string> toks(n_tokens);
+        std::vector<uint32_t> id(ids, ids + n_tokens);
+        for (uint32_t i = 0; i < n_tokens; ++i) toks[i].assign((const char*)blob + tok_offsets[i], tok_offsets[i + 1] - tok_offsets[i]);
+        std::vector<std::pair<uint32_t, uint32_t>> mg(n_merges);
+        for (uint32_t i = 0; i < n_merges; ++i) mg[i] = {merges[2 * i], merges[2 * i + 1]};
+        ModelState& m = p->impl.model(model_key, true);
+        m.tokenizer.reset(new Tokenizer(toks, id, mg, collect_specials(special_strs, special_ids, n_special), dev, ms));
+        return SMGX_SUCCESS;
+    });
+}
 
 // H2D the ragged text and tokenise it on `lane`; returns the device token buffers (valid until the lane is reused).
 static void tokenize_on_lane(Policy& P, ModelState& m, Lane& lane, const uint8_t* text, const uint32_t* offsets, uint32_t n,
@@ -1724,7 +1754,7 @@ static void tokenize_on_lane(Policy& P, ModelState& m, Lane& lane, const uint8_t
     lane.d_text.reserve(std::max<uint32_t>(total, 1) + 16);
     lane.d_offsets.reserve(((size_t)n + 1) * 4);
     lane.d_toff.reserve(((size_t)n + 1) * 4);
-    lane.d_tokens.reserve((size_t)std::max<uint32_t>(total, 1) * m.tokenizer->growth() * 4 + 16);   // NFC can grow the text threefold
+    lane.d_tokens.reserve((size_t)std::max<uint32_t>(total, 1) * m.tokenizer->growth() * 4 + 16);   // growth(): most tokens per byte
     if (n == 0) return;
     if (total) SMGX_CUDA(cudaMemcpyAsync(lane.d_text.ptr, text + base, total, cudaMemcpyHostToDevice, lane.stream));
     SMGX_CUDA(cudaMemcpyAsync(lane.d_offsets.ptr, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, lane.stream));

@@ -371,6 +371,9 @@ __global__ void __launch_bounds__(256) bpe_lookup_kernel(BpeView v, const uint8_
     }
 }
 
+// kChar (SentencePiece-style BPE): the initial symbols are not the piece's bytes but what ms_symbolize_kernel left in the piece's slots of
+// tmp_ids (code-point ids and byte-fallback tokens, kInvalidTok between them), and the tiers go by symbol count, not byte length.
+template <bool kChar>
 __global__ void __launch_bounds__(256) bpe_merge_kernel(BpeView v, const uint8_t* __restrict__ text, const Piece* __restrict__ pieces,
                                                         const uint32_t* __restrict__ counters, const uint32_t* __restrict__ miss_short,
                                                         uint32_t* __restrict__ tmp_ids, uint32_t* __restrict__ totals) {
@@ -386,13 +389,18 @@ __global__ void __launch_bounds__(256) bpe_merge_kernel(BpeView v, const uint8_t
         const uint32_t i = pc.start, plen = pc.len;
         uint32_t m = plen;
         if (valid) {
-            for (uint32_t j = 0; j < plen; ++j) s_id[j][tid] = v.byte_token[text[i + j]];
-            for (uint32_t j = 0; j + 1 < plen; ++j) {
+            if constexpr (kChar) {
+                m = 0;
+                for (uint32_t j = 0; j < plen; ++j) { const uint32_t id = tmp_ids[i + j]; if (id != kInvalidTok) s_id[m++][tid] = id; }
+            } else {
+                for (uint32_t j = 0; j < plen; ++j) s_id[j][tid] = v.byte_token[text[i + j]];
+            }
+            for (uint32_t j = 0; j + 1 < m; ++j) {
                 const uint64_t pr = pair_lookup(v, s_id[j][tid], s_id[j + 1][tid]);
                 s_rank[j][tid] = (uint32_t)(pr >> 32); s_mid[j][tid] = (uint32_t)pr;
             }
         }
-        bool merging = valid && plen >= 2;
+        bool merging = valid && m >= 2;
         while (__any_sync(0xffffffffu, merging)) {
             if (merging) {
                 uint32_t best = kRankMax, bi = 0;
@@ -417,6 +425,21 @@ __global__ void __launch_bounds__(256) bpe_merge_kernel(BpeView v, const uint8_t
     }
 }
 
+// kChar: pack the symbols of a piece's slots tmp_ids[i .. i+plen) (kInvalidTok between them) into w[0 ..); w may be those slots themselves
+// (a lane writes at or below the index it read, and every read of a round precedes its writes).
+__device__ __forceinline__ void gather_symbols(const uint32_t* tmp_ids, uint32_t i, uint32_t plen, uint32_t* w, int lane) {
+    uint32_t written = 0;
+    for (uint32_t base = 0; base < plen; base += 32) {
+        const uint32_t j = base + lane;
+        const uint32_t id = j < plen ? tmp_ids[i + j] : kInvalidTok;
+        const unsigned bal = __ballot_sync(0xffffffffu, id != kInvalidTok);
+        if (id != kInvalidTok) w[written + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = id;
+        written += (uint32_t)__popc(bal);
+    }
+    __syncwarp();
+}
+
+template <bool kChar>
 __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t* __restrict__ text, const Piece* __restrict__ pieces,
                                                        const uint32_t* __restrict__ counters, const uint32_t* __restrict__ miss_long,
                                                        uint32_t* __restrict__ tmp_ids, uint64_t* __restrict__ tmp_rk, uint32_t* __restrict__ totals) {
@@ -428,10 +451,23 @@ __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t*
     for (uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += nw) {
         const Piece pc = pieces[miss_long[k]];
         const uint32_t i = pc.start, plen = pc.len;
+        uint32_t ns = plen;   // initial symbols
+        if constexpr (kChar) {
+            ns = 0;
+            for (uint32_t base = 0; base < plen; base += 32)
+                ns += (uint32_t)__popc(__ballot_sync(0xffffffffu, base + lane < plen && tmp_ids[i + base + lane] != kInvalidTok));
+        }
         uint32_t m;
-        if (plen <= 32) {
-            m = plen;
-            uint32_t id = (uint32_t)lane < plen ? v.byte_token[text[i + lane]] : 0;
+        if (ns <= 32) {
+            m = ns;
+            uint32_t id;
+            if constexpr (kChar) {
+                gather_symbols(tmp_ids, i, plen, s_id[wid], lane);
+                id = (uint32_t)lane < ns ? s_id[wid][lane] : 0;
+                __syncwarp();
+            } else {
+                id = (uint32_t)lane < plen ? v.byte_token[text[i + lane]] : 0;
+            }
             uint32_t nid = __shfl_down_sync(0xffffffffu, id, 1);
             uint32_t rank = kRankMax, mid = 0;
             if ((uint32_t)lane + 1 < m) { const uint64_t pr = pair_lookup(v, id, nid); rank = (uint32_t)(pr >> 32); mid = (uint32_t)pr; }
@@ -451,24 +487,33 @@ __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t*
                     if ((uint32_t)lane + 1 < m) { const uint64_t pr = pair_lookup(v, id, nid); rank = (uint32_t)(pr >> 32); mid = (uint32_t)pr; }
                 }
             }
-            if ((uint32_t)lane < plen) tmp_ids[i + lane] = (uint32_t)lane < m ? id : kInvalidTok;
-        } else if (plen <= kLongSyms) {
-            // 33 … kLongSyms bytes: symbols stay in place in shared memory, linked by next/prev indices (list order = index order, so
+            if constexpr (kChar) {
+                if ((uint32_t)lane < m) tmp_ids[i + lane] = id;
+                for (uint32_t j = m + lane; j < plen; j += 32) tmp_ids[i + j] = kInvalidTok;
+            } else {
+                if ((uint32_t)lane < plen) tmp_ids[i + lane] = (uint32_t)lane < m ? id : kInvalidTok;
+            }
+        } else if (ns <= kLongSyms) {
+            // 33 … kLongSyms symbols: symbols stay in place in shared memory, linked by next/prev indices (list order = index order, so
             // "leftmost" = smallest index); a merge unlinks one symbol and re-ranks two pairs; the minimum is a strided scan + 2 redux
             uint32_t* w_id = s_id[wid]; uint32_t* w_rank = s_rank[wid]; uint32_t* w_mid = s_mid[wid];
             uint16_t* w_nxt = s_nxt[wid]; uint16_t* w_prv = s_prv[wid];
-            for (uint32_t j = lane; j < plen; j += 32) { w_id[j] = v.byte_token[text[i + j]]; w_nxt[j] = (uint16_t)(j + 1); w_prv[j] = (uint16_t)(j ? j - 1 : 0xFFFF); }
+            if constexpr (kChar) gather_symbols(tmp_ids, i, plen, w_id, lane);
+            for (uint32_t j = lane; j < ns; j += 32) {
+                if constexpr (!kChar) w_id[j] = v.byte_token[text[i + j]];
+                w_nxt[j] = (uint16_t)(j + 1); w_prv[j] = (uint16_t)(j ? j - 1 : 0xFFFF);
+            }
             __syncwarp();
-            for (uint32_t j = lane; j < plen; j += 32) {
+            for (uint32_t j = lane; j < ns; j += 32) {
                 uint32_t rk = kRankMax, md = 0;
-                if (j + 1 < plen) { const uint64_t pr = pair_lookup(v, w_id[j], w_id[j + 1]); rk = (uint32_t)(pr >> 32); md = (uint32_t)pr; }
+                if (j + 1 < ns) { const uint64_t pr = pair_lookup(v, w_id[j], w_id[j + 1]); rk = (uint32_t)(pr >> 32); md = (uint32_t)pr; }
                 w_rank[j] = rk; w_mid[j] = md;
             }
             __syncwarp();
-            m = plen;
+            m = ns;
             for (;;) {
                 uint32_t best = kRankMax, bpos = 0xFFFFFFFFu;
-                for (uint32_t j = lane; j < plen; j += 32) { const uint32_t rk = w_rank[j]; if (rk < best) { best = rk; bpos = j; } }   // ascending j: leftmost per lane
+                for (uint32_t j = lane; j < ns; j += 32) { const uint32_t rk = w_rank[j]; if (rk < best) { best = rk; bpos = j; } }   // ascending j: leftmost per lane
                 const uint32_t rmin = __reduce_min_sync(0xffffffffu, best);
                 if (rmin == kRankMax) break;
                 const uint32_t b = __reduce_min_sync(0xffffffffu, best == rmin ? bpos : 0xFFFFFFFFu);
@@ -476,12 +521,12 @@ __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t*
                 __syncwarp();
                 if (lane == 0) {
                     w_id[b] = w_mid[b]; w_nxt[b] = (uint16_t)d; w_rank[c] = kRankMax; w_id[c] = kInvalidTok;
-                    if (d < plen) w_prv[d] = (uint16_t)b;
+                    if (d < ns) w_prv[d] = (uint16_t)b;
                 }
                 __syncwarp();
                 if (lane == 0) {
                     uint32_t rk = kRankMax, md = 0;
-                    if (d < plen) { const uint64_t pr = pair_lookup(v, w_id[b], w_id[d]); rk = (uint32_t)(pr >> 32); md = (uint32_t)pr; }
+                    if (d < ns) { const uint64_t pr = pair_lookup(v, w_id[b], w_id[d]); rk = (uint32_t)(pr >> 32); md = (uint32_t)pr; }
                     w_rank[b] = rk; w_mid[b] = md;
                 } else if (lane == 1 && a != 0xFFFF) {
                     const uint64_t pr = pair_lookup(v, w_id[a], w_id[b]);
@@ -491,9 +536,9 @@ __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t*
                 __syncwarp();
             }
             uint32_t written = 0;   // compact the surviving symbols to the front of the piece's slots
-            for (uint32_t base = 0; base < plen; base += 32) {
+            for (uint32_t base = 0; base < ns; base += 32) {
                 const uint32_t j = base + lane;
-                const bool alive = j < plen && w_id[j] != kInvalidTok;
+                const bool alive = j < ns && w_id[j] != kInvalidTok;
                 const unsigned bal = __ballot_sync(0xffffffffu, alive);
                 if (alive) tmp_ids[i + written + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = w_id[j];
                 written += (uint32_t)__popc(bal);
@@ -502,8 +547,10 @@ __global__ void __launch_bounds__(256) bpe_long_kernel(BpeView v, const uint8_t*
             __syncwarp();
         } else {
             m = 0;
+            if constexpr (kChar) gather_symbols(tmp_ids, i, plen, tmp_ids + i, lane);   // in place
             if (lane == 0) {
-                m = byte_pair_merge(v, text + i, plen, tmp_ids + i, tmp_rk + i);
+                if constexpr (kChar) m = merge_symbols(v, tmp_ids + i, ns, tmp_rk + i);
+                else m = byte_pair_merge(v, text + i, plen, tmp_ids + i, tmp_rk + i);
                 for (uint32_t j = i + m; j < i + plen; ++j) tmp_ids[j] = kInvalidTok;
             }
             m = __shfl_sync(0xffffffffu, m, 0);
@@ -712,6 +759,104 @@ __global__ void __launch_bounds__(256) nfc_write_kernel(const uint8_t* __restric
     }
 }
 
+// K1m: SentencePiece-style BPE (metaspace.cuh), only for a tokenizer loaded with smgx_tokenizer_load_bpe_metaspace.  Like the NFC stage
+// it runs after the specials are resolved on the raw text and writes a normalized ragged copy of the batch (text, flags, the specials'
+// ids); a stretch of L raw bytes becomes at most 3L + 3 ≤ 6L bytes and at most L + 1 ≤ 2L initial symbols.  Then:
+//   ms_count_kernel      thread per raw byte: output bytes; chunk_sum (per 256-byte chunk) and nlen (per request) collect them
+//   scan_counts_kernel   normalized request lengths → offsets of the normalized batch
+//   ms_write_kernel      thread per raw byte: writes its bytes at (earlier chunks of the request + exclusive scan within the chunk)
+//   ms_symbolize_kernel  thread per normalized byte: a code point's initial symbols into its slots of tmp_ids (ms_symbolize), and flags = 1
+//                        where a piece starts (ms_piece_start)
+//   ms_emit_kernel       thread per piece start: counts the piece's symbols up to the next start, a special or the request end; a
+//                        single symbol is already its token, longer pieces go to the merge kernels' lists by symbol count
+// and bpe_merge_kernel<true> / bpe_long_kernel<true> merge them.
+__global__ void __launch_bounds__(256) ms_count_kernel(MetaspaceMode mm, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                       uint32_t first_byte, const uint8_t* __restrict__ flags, uint32_t* __restrict__ chunk_sum,
+                                                       uint32_t* __restrict__ nlen) {
+    __shared__ uint32_t s_w[8];
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t cstart = beg + blockIdx.x * blockDim.x;
+    if (cstart >= rend) return;   // CTA-uniform
+    const uint32_t i = cstart + threadIdx.x;
+    const uint32_t sum = block_sum_256(i < rend ? ms_out_len(mm, text, flags, i, beg) : 0, s_w);
+    if (threadIdx.x == 0) {
+        chunk_sum[cstart - first_byte] = sum;
+        atomicAdd(&nlen[r], sum);
+    }
+}
+
+__global__ void __launch_bounds__(256) ms_write_kernel(MetaspaceMode mm, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                       uint32_t first_byte, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ tmp_ids,
+                                                       const uint32_t* __restrict__ chunk_sum, const uint32_t* __restrict__ noff,
+                                                       uint8_t* __restrict__ ntext, uint8_t* __restrict__ nflags, uint32_t* __restrict__ nids) {
+    __shared__ uint32_t s_w[8];
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t cstart = beg + blockIdx.x * blockDim.x;
+    if (cstart >= rend) return;
+    const uint32_t i = cstart + threadIdx.x;
+    uint32_t pre = 0;   // output bytes of the request's earlier chunks
+    for (uint32_t c = threadIdx.x; c < blockIdx.x; c += blockDim.x) pre += chunk_sum[beg + c * 256 - first_byte];
+    const uint32_t base = block_sum_256(pre, s_w);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t len = i < rend ? ms_out_len(mm, text, flags, i, beg) : 0;
+    uint32_t inc = len;   // inclusive scan within the warp, then across the 8 warps
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
+    if (lane == 31) s_w[wid] = inc;
+    __syncthreads();
+    uint32_t before = 0;
+    for (int w = 0; w < wid; ++w) before += s_w[w];
+    if (i < rend) {
+        const uint32_t o = noff[r] + base + before + inc - len;
+        const uint8_t fl = flags[i];
+        ms_out_write(mm, text, flags, i, beg, ntext + o);
+        for (uint32_t j = 0; j < len; ++j) nflags[o + j] = fl >= 2 ? fl : 0;
+        if (fl >= 2) nids[o] = tmp_ids[i];
+    }
+}
+
+__global__ void __launch_bounds__(256) ms_symbolize_kernel(BpeView v, uint32_t split, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
+                                                           uint8_t* __restrict__ flags, uint32_t* __restrict__ tmp_ids) {
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t i = beg + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rend || flags[i] >= 2 || (text[i] & 0xC0) == 0x80) return;
+    uint32_t ns;
+    ms_symbolize(v, text, i, rend, tmp_ids + i, &ns);
+    if (ms_piece_start(text, flags, i, beg, split)) flags[i] = 1;   // neighbours only test flags >= 2: 0 → 1 does not change their answer
+}
+
+__global__ void __launch_bounds__(256) ms_emit_kernel(const uint32_t* __restrict__ offsets, const uint8_t* __restrict__ flags,
+                                                      const uint32_t* __restrict__ tmp_ids, Piece* __restrict__ pieces, uint32_t* __restrict__ counters,
+                                                      uint32_t* __restrict__ totals, uint32_t* __restrict__ miss_short, uint32_t* __restrict__ miss_long) {
+    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t cstart = beg + blockIdx.x * blockDim.x;
+    if (cstart >= rend) return;   // CTA-uniform: the warps below stay whole
+    const uint32_t i = cstart + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    uint32_t ns = 0, j = i;
+    if (i < rend && flags[i] == 1) {
+        for (j = i; j < rend && (j == i || flags[j] == 0); ++j) ns += tmp_ids[j] != kInvalidTok;
+    }
+    const int kind = ns == 1 ? 3 : ns > kSmemSyms ? 2 : ns ? 1 : 0;   // 3: one symbol, already the token
+    const unsigned one = __ballot_sync(0xffffffffu, kind == 3);
+    if (lane == 0 && one) atomicAdd(&totals[r], (uint32_t)__popc(one));
+#pragma unroll
+    for (int k = 1; k <= 2; ++k) {
+        const unsigned bal = __ballot_sync(0xffffffffu, kind == k);
+        if (!bal) continue;
+        const int leader = __ffs((int)bal) - 1;
+        uint32_t pbase = 0, lbase = 0;
+        if (lane == leader) { pbase = atomicAdd(&counters[0], (uint32_t)__popc(bal)); lbase = atomicAdd(&counters[k], (uint32_t)__popc(bal)); }
+        pbase = __shfl_sync(0xffffffffu, pbase, leader);
+        lbase = __shfl_sync(0xffffffffu, lbase, leader);
+        if (kind == k) {
+            const uint32_t rank = (uint32_t)__popc(bal & ((1u << lane) - 1u));
+            pieces[pbase + rank] = Piece{i, j - i, r};
+            (k == 1 ? miss_short : miss_long)[lbase + rank] = pbase + rank;
+        }
+    }
+}
+
 uint32_t pow2_at_least(uint64_t x) { uint32_t p = 1024; while (p < x) p <<= 1; return p; }
 
 std::string b64decode(const std::string& in) {
@@ -768,6 +913,12 @@ Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<u
     : device_(device), pretok_(pretok), nfc_(nfc) {
     build(tokens, ids, &merges, ignore_merges, specials);
 }
+Tokenizer::Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
+                     const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, MetaspaceMode ms)
+    : device_(device), ms_(ms) {
+    ms_.on = 1;
+    build(tokens, ids, &merges, false, specials);
+}
 
 void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ranks, const std::vector<std::pair<uint32_t, uint32_t>>* merges,
                       bool whole_piece, const std::vector<std::pair<std::string, uint32_t>>& specials) {
@@ -787,10 +938,20 @@ void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<
 
     std::vector<uint32_t> byte_token(256);
     for (int b = 0; b < 256; ++b) {
+        if (ms_.on) {   // byte fallback: `tokenizers` looks up format!("<{b:#04X}>")
+            char name[8];
+            snprintf(name, sizeof(name), "<0x%02X>", b);
+            auto it = enc.find(name);
+            if (it == enc.end()) throw Error(SMGX_TOKENIZATION_ERROR, std::string("vocabulary lacks the byte-fallback token ") + name);
+            byte_token[b] = it->second;
+            continue;
+        }
         auto it = enc.find(std::string(1, (char)b));
         if (it == enc.end()) throw Error(SMGX_TOKENIZATION_ERROR, "vocabulary lacks the single-byte token " + std::to_string(b));
         byte_token[b] = it->second;
     }
+    static const std::string kMeta = "\xE2\x96\x81";   // ▁
+    if (ms_.on && !enc.count(kMeta)) throw Error(SMGX_TOKENIZATION_ERROR, "vocabulary lacks the token \"\xE2\x96\x81\" (U+2581)");
     // blob of token bytes + piece table keyed by the bytes
     std::vector<uint8_t> blob;
     std::vector<PieceSlot> pieces(pow2_at_least(tokens.size() * 2), PieceSlot{0, 0, 0, 0, 0});
@@ -827,6 +988,13 @@ void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<
             if (l == by_id.end() || r == by_id.end()) throw Error(SMGX_TOKENIZATION_ERROR, "merge refers to an unknown token id");
             auto t = enc.find(*l->second + *r->second);
             if (t == enc.end()) throw Error(SMGX_TOKENIZATION_ERROR, "merge result is not in the vocabulary");
+            // Pieces are cut before every ▁ that follows another character.  Exact unless a merge joins a symbol that does not end in ▁
+            // (a character, or a byte token) to one that starts with ▁: only such a pair can straddle a cut (DESIGN §4c).
+            const std::string &ls = *l->second, &rs = *r->second;
+            if (ms_.on && !ms_.split && rs.compare(0, kMeta.size(), kMeta) == 0 &&
+                !(ls.size() >= kMeta.size() && ls.compare(ls.size() - kMeta.size(), kMeta.size(), kMeta) == 0))
+                throw Error(SMGX_TOKENIZATION_ERROR, "merge " + std::to_string(k) + " (\"" + ls + "\", \"" + rs + "\") joins a symbol that does not end "
+                            "in \xE2\x96\x81 to one that starts with \xE2\x96\x81: the text cannot be cut into independent pieces at \xE2\x96\x81");
             pair_list.push_back({((uint64_t)l->first << 32) | r->first, (uint32_t)k, t->second});
         }
     }
@@ -905,10 +1073,13 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
     if (!device_) throw Error(SMGX_DEVICE_ERROR, "tokenizer was loaded without a device (host-mirror policy): no GPU path, no CPU fallback");
     if (n == 0) return;
     const uint32_t raw = total_bytes - first_byte;
-    if (nfc_) SMGX_REQUIRE(3ull * raw < (1ull << 31) && 3ull * max_len < (1ull << 31), "text batch too large for the normalizer");
-    // bytes the pre-tokenizer and BPE see: the raw text, or its normalized copy (at most 3x, at absolute offsets from 0)
-    const uint32_t span = nfc_ ? 3 * raw : raw;
-    const uint32_t span_end = nfc_ ? span : total_bytes;
+    const bool norm = nfc_ || ms_.on;
+    const uint64_t tg = text_growth();
+    if (norm) SMGX_REQUIRE(tg * raw < (1ull << 31) && tg * max_len < (1ull << 31), "text batch too large for the normalizer");
+    // bytes the pre-tokenizer and BPE see: the raw text, or its normalized copy (at most text_growth() times as long, at absolute
+    // offsets from 0)
+    const uint32_t span = norm ? (uint32_t)(tg * raw) : raw;
+    const uint32_t span_end = norm ? span : total_bytes;
     sc.flags.reserve(std::max<uint32_t>(total_bytes, 1));
     sc.tmp_ids.reserve((size_t)std::max<uint32_t>(total_bytes, 1) * 4);
     sc.tmp_rk.reserve((size_t)std::max<uint32_t>(std::max(total_bytes, span_end), 1) * 8);
@@ -976,9 +1147,49 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
             flags = b + o_flags;
             tmp_ids = (uint32_t*)(b + o_ids);
             len_bound = 3 * max_len;
+        } else if (ms_.on && max_len) {
+            // scratch, 16-byte aligned slices of one allocation: normalized text / flags / ids (6 per raw byte), chunk sums (per raw
+            // byte), per request: normalized length and offsets
+            const size_t R = std::max<uint32_t>(raw, 1);
+            size_t at = 0;
+            auto slice = [&at](size_t bytes) { const size_t o = at; at = (at + bytes + 15) / 16 * 16; return o; };
+            const size_t o_text = slice(6 * R), o_flags = slice(6 * R), o_ids = slice(6 * R * 4), o_chunk = slice(R * 4),
+                         o_req = slice(((size_t)2 * n + 1) * 4);
+            sc.nfc.reserve(at);
+            uint8_t* b = sc.nfc.as<uint8_t>();
+            uint32_t* nlen = (uint32_t*)(b + o_req);
+            uint32_t* noff = nlen + n;
+            uint32_t* chunk_sum = (uint32_t*)(b + o_chunk);   // indexed from first_byte
+            SMGX_CUDA(cudaMemsetAsync(nlen, 0, (size_t)n * 4, stream));
+            ms_count_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, first_byte, flags, chunk_sum, nlen);
+            scan_counts_kernel<<<1, 1024, 0, stream>>>(nlen, n, noff);
+            ms_write_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, first_byte, flags, tmp_ids, chunk_sum, noff, b + o_text, b + o_flags,
+                                                       (uint32_t*)(b + o_ids));
+            SMGX_CUDA(cudaGetLastError());
+            *launches += 3;
+            text = b + o_text;
+            offsets = noff;
+            flags = b + o_flags;
+            tmp_ids = (uint32_t*)(b + o_ids);
+            len_bound = 6 * max_len;
         }
         SMGX_CUDA(cudaMemsetAsync(sc.n_pieces.ptr, 0, 16, stream));
-        if (max_len) {
+        if (max_len && ms_.on) {
+            // segmenter + symbolizer instead of the pre-tokenizer and the whole-piece lookup, then the merge tiers by symbol count
+            const dim3 gridn((len_bound + 255) / 256, n);   // CTAs past a request's normalized end return at once
+            const unsigned sms = current_sm_count();
+            const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)span / 2 + 255) / 256 + 1, sms * 16ull);
+            uint32_t* cnt = sc.n_pieces.as<uint32_t>();
+            uint32_t* miss_short = sc.miss.as<uint32_t>();
+            uint32_t* miss_long = miss_short + span + 1;
+            ms_symbolize_kernel<<<gridn, 256, 0, stream>>>(dview_, ms_.split, text, offsets, flags, tmp_ids);
+            ms_emit_kernel<<<gridn, 256, 0, stream>>>(offsets, flags, tmp_ids, sc.pieces.as<Piece>(), cnt, sc.totals.as<uint32_t>(), miss_short, miss_long);
+            bpe_merge_kernel<true><<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_short, tmp_ids, sc.totals.as<uint32_t>());
+            bpe_long_kernel<true><<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_long, tmp_ids,
+                                                                          sc.tmp_rk.as<uint64_t>(), sc.totals.as<uint32_t>());
+            SMGX_CUDA(cudaGetLastError());
+            *launches += 4;
+        } else if (max_len) {
             const dim3 gridp((len_bound + 255) / 256, n);   // with NFC: CTAs past a request's normalized end find an empty window
             if (pretok_ == Pretok::R50k)
                 pretokenize_kernel<Pretok::R50k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
@@ -995,9 +1206,9 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
             uint32_t* miss_short = sc.miss.as<uint32_t>();
             uint32_t* miss_long = miss_short + span + 1;
             bpe_lookup_kernel<<<grid, 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, tmp_ids, sc.totals.as<uint32_t>(), miss_short, miss_long);
-            bpe_merge_kernel<<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_short, tmp_ids, sc.totals.as<uint32_t>());
-            bpe_long_kernel<<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_long, tmp_ids,
-                                                                    sc.tmp_rk.as<uint64_t>(), sc.totals.as<uint32_t>());
+            bpe_merge_kernel<false><<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_short, tmp_ids, sc.totals.as<uint32_t>());
+            bpe_long_kernel<false><<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_long, tmp_ids,
+                                                                           sc.tmp_rk.as<uint64_t>(), sc.totals.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             *launches += 3;
         }

@@ -8,6 +8,7 @@
 
 #include "bpe.cuh"
 #include "common.h"
+#include "metaspace.cuh"
 #include "nfc.cuh"
 
 namespace smgx {
@@ -22,6 +23,12 @@ public:
     // nfc: the tokenizer.json normalizer is NFC (nfc.cuh); the text between specials is normalized before it is split.
     Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
               bool ignore_merges, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, Pretok pretok, bool nfc = false);
+    // SentencePiece-style BPE with byte fallback (metaspace.cuh): tokens are raw UTF-8 strings, the byte-fallback tokens are the vocabulary
+    // entries "<0x00>" … "<0xFF>"; `ms` says how spaces become ▁ and where pieces start.  Refuses (SMGX_TOKENIZATION_ERROR) a vocabulary
+    // without ▁ or one of the byte tokens, and — when pieces are cut only at ▁ after another character — a merge that could join
+    // two pieces (DESIGN §4c).
+    Tokenizer(const std::vector<std::string>& tokens, const std::vector<uint32_t>& ids, const std::vector<std::pair<uint32_t, uint32_t>>& merges,
+              const std::vector<std::pair<std::string, uint32_t>>& specials, bool device, MetaspaceMode ms);
     ~Tokenizer();
     static Tokenizer* from_tiktoken_file(const std::string& path, const std::vector<std::pair<std::string, uint32_t>>& specials, bool device,
                                          Pretok pretok);
@@ -29,13 +36,16 @@ public:
     BpeView view() const { return dview_; }
     uint32_t vocab_size() const { return vocab_size_; }
     uint32_t n_pairs() const { return n_pairs_; }
-    // Most bytes of normalized text (and so most tokens) per byte of input: 3 with NFC (U+1D160 → three code points), else 1.
-    uint32_t growth() const { return nfc_ ? 3u : 1u; }
+    // Most tokens per byte of input: 3 with NFC (U+1D160 → three code points), 2 for SentencePiece-style BPE (a stretch of L bytes has at
+    // most L + 1 initial symbols), else 1.
+    uint32_t growth() const { return nfc_ ? 3u : ms_.on ? 2u : 1u; }
+    // Most bytes of normalized text per byte of input: 3 with NFC, 6 for SentencePiece-style BPE (" " → "▁▁" at a stretch start), else 1.
+    uint32_t text_growth() const { return nfc_ ? 3u : ms_.on ? 6u : 1u; }
 
-    // Scratch needed for a batch of `total_bytes` of text and `n` requests; `nfc` holds the normalization stage's buffers.
+    // Scratch needed for a batch of `total_bytes` of text and `n` requests; `nfc` holds the normalization stage's buffers (NFC or ▁).
     struct Scratch { DevBuf flags, tmp_ids, tmp_rk, totals, pieces, n_pieces, miss, nfc; };
 
-    // Enqueue [NFC +] pre-tokenise + BPE + compaction on `stream`.
+    // Enqueue [NFC or ▁ normalization +] pre-tokenise + BPE + compaction on `stream`.
     //   d_text/d_offsets (n+1): ragged UTF-8; d_tokens: capacity ≥ growth() × (total_bytes - first_byte) u32; d_tok_offsets: n+1 u32 (written).
     // Text bytes live at d_text[first_byte .. total_bytes) (absolute offsets as given in d_offsets).
     // `max_len` = longest request in bytes (sizes the 2-D grids).
@@ -50,6 +60,7 @@ private:
     bool device_ = false;
     Pretok pretok_ = Pretok::Cl100k;
     bool nfc_ = false;
+    MetaspaceMode ms_{};
     NfcView nview_{};
     DevBuf d_byte_token_, d_pairs_, d_pieces_, d_blob_, d_specials_, d_uni_lo_, d_uni_hi_, d_uni_cls_, d_nfc_;
 };

@@ -498,17 +498,66 @@ def _hf_normalizer(norm):
     raise ValueError("tokenizer.json: the only normalizer supported on the GPU path is NFC (alone or as a one-element Sequence)")
 
 
+METASPACE = "▁"   # ▁, SentencePiece's space
+_PREPEND_SCHEMES = {"never": _lib.PREPEND_NEVER, "first": _lib.PREPEND_FIRST, "always": _lib.PREPEND_ALWAYS}
+
+
+def _hf_sentencepiece(j):
+    """The two SentencePiece-style tokenizer.json shapes → (smgx_sp_shape, smgx_prepend_scheme, split), or None when the file has neither
+    the legacy normalizer nor a Metaspace pre_tokenizer.  A file that has one of them in any other form is refused with ValueError.
+      legacy     normalizer Sequence[Prepend("▁"), Replace(String " " → "▁")], pre_tokenizer null (Llama 2, Mistral v0.1/v0.2, TinyLlama);
+      metaspace  normalizer null, pre_tokenizer Metaspace(replacement "▁", prepend_scheme, split), read as the `tokenizers` crate reads it:
+                 prepend_scheme defaults to "always", split to true, and add_prefix_space = false is only valid with prepend_scheme
+                 "never" (which it then means)."""
+    norm, pre = j.get("normalizer"), j.get("pre_tokenizer")
+    steps = norm.get("normalizers", []) if norm and norm.get("type") == "Sequence" else [norm] if norm else []
+    if any(s.get("type") in ("Prepend", "Replace") for s in steps):
+        if [s.get("type") for s in steps] != ["Prepend", "Replace"]:
+            return None   # e.g. Prepend alone: refused by _hf_normalizer
+        p, r = steps
+        if p.get("prepend") != METASPACE or r.get("pattern") != {"String": " "} or r.get("content") != METASPACE:
+            raise ValueError("tokenizer.json: the SentencePiece-style normalizer must be Sequence[Prepend(\"▁\"), Replace(String \" \" → \"▁\")]")
+        if pre is not None:
+            raise ValueError("tokenizer.json: the Prepend + Replace normalizer is supported with pre_tokenizer null only")
+        return _lib.SP_LEGACY, _lib.PREPEND_ALWAYS, 0
+    if not pre or pre.get("type") != "Metaspace":
+        return None
+    if norm is not None:
+        raise ValueError("tokenizer.json: a Metaspace pre_tokenizer is supported with normalizer null only")
+    if pre.get("replacement") != METASPACE:
+        raise ValueError("tokenizer.json: the Metaspace replacement must be \"▁\" (U+2581)")
+    scheme = pre.get("prepend_scheme", "always")
+    if scheme not in _PREPEND_SCHEMES:
+        raise ValueError(f"tokenizer.json: unknown Metaspace prepend_scheme {scheme!r}")
+    if pre.get("add_prefix_space") is False and scheme != "never":
+        raise ValueError("tokenizer.json: Metaspace add_prefix_space = false does not match prepend_scheme " + repr(scheme))
+    split = pre.get("split", True)
+    if not isinstance(split, bool):
+        raise ValueError("tokenizer.json: Metaspace split must be true or false")
+    return _lib.SP_METASPACE, _PREPEND_SCHEMES[scheme], int(split)
+
+
 class HuggingFaceTokenizer(TiktokenTokenizer):
-    """tokenizer::HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs) for the byte-level BPE family the GPU path covers:
-    tokenizer.json with no normalizer or NFC, either Split(Llama-3 / cl100k or Qwen2 regex, Isolated) + ByteLevel(use_regex=False) or
-    GPT-2's ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk / byte_fallback.  Anything else is
-    refused loudly — there is no CPU tokenizer behind this."""
+    """tokenizer::HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs) for the BPE families the GPU path covers:
+    - byte-level BPE: tokenizer.json with no normalizer or NFC, either Split(Llama-3 / cl100k or Qwen2 regex, Isolated) +
+      ByteLevel(use_regex=False) or GPT-2's ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk /
+      byte_fallback;
+    - SentencePiece-style BPE (Llama 2, CodeLlama, Mistral, Mixtral, TinyLlama): the legacy normalizer Sequence[Prepend("▁"),
+      Replace(" " → "▁")] without a pre_tokenizer, or Metaspace(replacement "▁") without a normalizer (_hf_sentencepiece); model BPE with
+      byte_fallback = true, the 256 <0xXX> tokens and "▁" in the vocabulary, ignore_merges = false, no dropout / continuing_subword_prefix /
+      end_of_word_suffix.  Vocabulary strings are raw UTF-8.  The load also refuses a vocabulary whose merges would not let the GPU cut a
+      stretch into pieces at ▁ (smgx_tokenizer_load_bpe_metaspace); the message names the merge.
+    Anything else is refused loudly with ValueError — there is no CPU tokenizer behind this."""
 
     def __init__(self, handle: _Handle, model: str, path: str):   # noqa: D401 — does not call the tiktoken loader
         import json
         self.h, self.model = handle, model.encode()
         j = json.load(open(path, encoding="utf-8"))
         mdl = j.get("model") or {}
+        sp = _hf_sentencepiece(j)
+        if sp is not None:
+            self._load_sentencepiece(j, mdl, sp)
+            return
         if mdl.get("type") != "BPE" or mdl.get("dropout") or mdl.get("unk_token") or mdl.get("byte_fallback") or \
                 mdl.get("continuing_subword_prefix") or mdl.get("end_of_word_suffix"):
             raise ValueError("tokenizer.json: only plain byte-level BPE models are supported on the GPU path")
@@ -528,6 +577,15 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         offs = np.zeros(len(toks) + 1, dtype=np.uint32)
         np.cumsum([len(t) for t in toks], out=offs[1:])
         blob = np.frombuffer(b"".join(toks), dtype=np.uint8).copy()
+        strs, sp_ids, n_added = self._added_tokens(j, norm != _lib.NORMALIZER_NONE)
+        self.growth = 3 if norm != _lib.NORMALIZER_NONE else 1   # NFC can grow text threefold
+        mg = _u32(merges)
+        self.h.call("smgx_tokenizer_load_bpe_merges_norm", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
+                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), n_added, pretok, norm)
+
+    @staticmethod
+    def _added_tokens(j, normalizer: bool):
+        """added_tokens → (C strings, ids, count) for the loaders, or ValueError for the kinds the GPU path does not implement."""
         added = [(a["content"], a["id"]) for a in j.get("added_tokens", [])]
         for a in j.get("added_tokens", []):
             if a.get("lstrip") or a.get("rstrip") or a.get("single_word"):
@@ -538,14 +596,38 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
             raise ValueError("tokenizer.json: added tokens with mixed `normalized` values are not supported")
         # With a normalizer, added tokens marked normalized are matched on the normalized text — a second pass the GPU path does not
         # implement.  Those marked normalized = false are cut from the raw text first, which is what the GPU path does.
-        if norm != _lib.NORMALIZER_NONE and any(a.get("normalized", False) for a in j.get("added_tokens", [])):
+        if normalizer and any(a.get("normalized", False) for a in j.get("added_tokens", [])):
             raise ValueError("tokenizer.json: added tokens with normalized = true are not supported together with a normalizer")
-        self.growth = 3 if norm != _lib.NORMALIZER_NONE else 1   # NFC can grow text threefold
         strs = (C.c_char_p * max(len(added), 1))(*[k.encode() for k, _ in added]) if added else None
-        sp_ids = _u32([v for _, v in added])
-        mg = _u32(merges)
-        self.h.call("smgx_tokenizer_load_bpe_merges_norm", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
-                    1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), len(added), pretok, norm)
+        return strs, _u32([v for _, v in added]), len(added)
+
+    def _load_sentencepiece(self, j, mdl, sp):
+        if mdl.get("type") != "BPE" or mdl.get("byte_fallback") is not True or mdl.get("dropout") is not None or mdl.get("ignore_merges") or \
+                mdl.get("continuing_subword_prefix") is not None or mdl.get("end_of_word_suffix") is not None:
+            raise ValueError("tokenizer.json: a SentencePiece-style model must be BPE with byte_fallback = true, ignore_merges = false and "
+                             "no dropout / continuing_subword_prefix / end_of_word_suffix")
+        vocab = mdl["vocab"]
+        missing = [t for t in [f"<0x{b:02X}>" for b in range(256)] + [METASPACE] if t not in vocab]
+        if missing:
+            raise ValueError(f"tokenizer.json: the vocabulary lacks {missing[0]!r} (byte fallback needs <0x00> … <0xFF>, and ▁ must be a token)")
+        toks = [s.encode("utf-8") for s in vocab]   # raw UTF-8: no byte-level mapping
+        merges = []
+        for m in mdl.get("merges", []):
+            a, b = m.split(" ") if isinstance(m, str) else m
+            merges += [vocab[a], vocab[b]]
+        offs = np.zeros(len(toks) + 1, dtype=np.uint32)
+        np.cumsum([len(t) for t in toks], out=offs[1:])
+        blob = np.frombuffer(b"".join(toks), dtype=np.uint8).copy()
+        strs, sp_ids, n_added = self._added_tokens(j, sp[0] == _lib.SP_LEGACY)
+        self.growth = 2   # a stretch of L bytes has at most L + 1 initial symbols
+        ids, mg = _u32(list(vocab.values())), _u32(merges)
+        try:
+            self.h.call("smgx_tokenizer_load_bpe_metaspace", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
+                        strs, _p(sp_ids), n_added, *sp)
+        except _lib.SmgxError as e:
+            if e.code != _lib.TOKENIZATION_ERROR:
+                raise
+            raise ValueError(f"tokenizer.json: {e}") from e
 
 
 TREE_BATCH_MODES = {"sequential": 0, "snapshot": 1}   # smgx_tree_batch_mode (include/smgx.h)
