@@ -11,12 +11,29 @@ namespace smgx {
 
 namespace {
 
-// 32-byte records (Slot / MultiNode): two threads per record, 16 B each → coalesced 32 B sector writes.
+// 32-byte records (Slot / MultiNode): two threads per record, 16 B each → coalesced 32 B sector writes.  For slots (tags != nullptr)
+// the thread that writes the first half (content, pos, state) writes the slot's tag as well.
 __global__ void scatter32_kernel(uint4* __restrict__ dst, const uint32_t* __restrict__ idx, const uint4* __restrict__ src,
-                                 uint32_t n) {
+                                 uint32_t n, uint8_t* __restrict__ tags) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t rec = t >> 1, half = t & 1;
-    if (rec < n) dst[(size_t)idx[rec] * 2 + half] = src[(size_t)rec * 2 + half];
+    if (rec >= n) return;
+    const uint32_t i = idx[rec];
+    const uint4 r = src[(size_t)rec * 2 + half];
+    dst[(size_t)i * 2 + half] = r;
+    if (tags && half == 0) tags[i] = slot_tag(r.w, r.z, (uint64_t)r.x | ((uint64_t)r.y << 32));
+}
+// every tag from the slots after a bulk upload; one thread per 4 slots writes one u32 of tags
+__global__ void derive_tags_kernel(const uint4* __restrict__ slots, uint32_t* __restrict__ tags, uint32_t n4) {
+    uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n4) return;
+    uint32_t w = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint4 r = slots[((size_t)t * 4 + k) * 2];
+        w |= (uint32_t)slot_tag(r.w, r.z, (uint64_t)r.x | ((uint64_t)r.y << 32)) << (8 * k);
+    }
+    tags[t] = w;
 }
 __global__ void scatter_rows_kernel(uint64_t* __restrict__ dst, const uint32_t* __restrict__ idx, const uint64_t* __restrict__ src,
                                     uint32_t n, uint32_t words) {
@@ -36,7 +53,7 @@ EventIndex::EventIndex(uint32_t jump_size) : jump_(jump_size) {
 }
 
 EventIndex::~EventIndex() {
-    d_slots_.release(); d_rows_.release(); d_multi_.release(); d_tree_.release(); d_stage_.release(); stage_.release();
+    d_slots_.release(); d_rows_.release(); d_multi_.release(); d_tree_.release(); d_tags_.release(); d_stage_.release(); stage_.release();
     if (stage_done_) cudaEventDestroy(stage_done_);
 }
 
@@ -353,7 +370,12 @@ EventIndexView EventIndex::flush(cudaStream_t stream, uint64_t* launches) {
         d_slots_.reserve(slots_.size() * sizeof(Slot));
         d_rows_.reserve(std::max<size_t>(rows_.capacity(), 1) * sizeof(uint64_t));
         d_multi_.reserve(std::max<size_t>(multi_.capacity(), 1) * sizeof(MultiNode));
+        d_tags_.reserve(slots_.size());
         SMGX_CUDA(cudaMemcpyAsync(d_slots_.ptr, slots_.data(), slots_.size() * sizeof(Slot), cudaMemcpyHostToDevice, stream));
+        const uint32_t n4 = (uint32_t)(slots_.size() / 4);   // capacity: a power of two ≥ 1024
+        derive_tags_kernel<<<(n4 + 255) / 256, 256, 0, stream>>>(d_slots_.as<uint4>(), d_tags_.as<uint32_t>(), n4);
+        SMGX_CUDA(cudaGetLastError());
+        ++*launches;
         if (!rows_.empty())
             SMGX_CUDA(cudaMemcpyAsync(d_rows_.ptr, rows_.data(), rows_.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
         if (!multi_.empty())
@@ -384,12 +406,12 @@ EventIndexView EventIndex::flush(cudaStream_t stream, uint64_t* launches) {
         char* ds = d_stage_.as<char>();
         if (ns) {
             scatter32_kernel<<<(unsigned)((ns * 2 + 255) / 256), 256, 0, stream>>>(d_slots_.as<uint4>(), (const uint32_t*)(ds + off_si),
-                                                                                 (const uint4*)(ds + off_sr), (uint32_t)ns);
+                                                                                 (const uint4*)(ds + off_sr), (uint32_t)ns, d_tags_.as<uint8_t>());
             ++*launches;
         }
         if (nm) {
             scatter32_kernel<<<(unsigned)((nm * 2 + 255) / 256), 256, 0, stream>>>(d_multi_.as<uint4>(), (const uint32_t*)(ds + off_mi),
-                                                                                 (const uint4*)(ds + off_mr), (uint32_t)nm);
+                                                                                 (const uint4*)(ds + off_mr), (uint32_t)nm, nullptr);
             ++*launches;
         }
         if (nr) {
@@ -413,6 +435,7 @@ EventIndexView EventIndex::flush(cudaStream_t stream, uint64_t* launches) {
     v.rows = d_rows_.as<uint64_t>();
     v.multi = d_multi_.as<MultiNode>();
     v.tree_sizes = d_tree_.as<uint64_t>();
+    v.tags = d_tags_.as<uint8_t>();
     v.mask = mask_;
     v.words = words_;
     v.n_workers = (uint32_t)tree_sizes_.size();

@@ -11,6 +11,13 @@
 //   rows   [n_rows][words] u64                                 worker bitsets (words = ceil(workers/64) → pow2, ≤ 32)
 //   multi  { u64 prefix_hash; u64 payload; u32 next; ... }     32 B nodes; one per distinct prefix hash
 //   tree_sizes[worker] u64                                     event_tree.rs:264
+//   tags   [capacity] u8                                       one byte per slot, derived on the device from the slots: 0 empty,
+//                                                              1 tombstone, tag_of(pos, content) ∈ 2..255 for a live key
+//
+// The slots are far larger than L2 (32 B each at ≤ 25 % load: 128 MiB for 1 M entries, most 128 B lines holding a live slot), so a
+// probe that reads a slot only to find a different key or an empty one is an HBM round trip that carries one bit.  The tag array is
+// 1 B per slot (4 MiB at 4 M slots) and stays in L2: a collision chain is walked in the tags, and a slot is read only where the tag
+// matches, then its full key is compared.
 //
 // Writers (apply_stored / apply_removed / apply_cleared / remove_worker, event_tree.rs:305-435) run on the host
 // against an identical host mirror and record dirty slots; flush() pushes them to the device with one scatter
@@ -52,15 +59,25 @@ struct EventIndexView {
     const uint64_t* rows;
     const MultiNode* multi;
     const uint64_t* tree_sizes;
+    const uint8_t* tags; // one tag per slot (see above)
     uint32_t mask;       // capacity - 1
     uint32_t words;      // u64 words per worker bitset
     uint32_t n_workers;  // interned workers
     uint32_t jump;       // jump_size (event_tree.rs:270)
 };
 
-__host__ __device__ inline uint32_t slot_hash(uint32_t pos, uint64_t content) {
-    uint64_t h = (content ^ ((uint64_t)pos * 0x9E3779B97F4A7C15ULL)) * 0xD6E8FEB86659FD93ULL;
-    return (uint32_t)(h >> 32);
+__host__ __device__ inline uint64_t key_hash(uint32_t pos, uint64_t content) {
+    return (content ^ ((uint64_t)pos * 0x9E3779B97F4A7C15ULL)) * 0xD6E8FEB86659FD93ULL;
+}
+// home slot: the high half of the key hash (masked to the capacity)
+__host__ __device__ inline uint32_t slot_hash(uint32_t pos, uint64_t content) { return (uint32_t)(key_hash(pos, content) >> 32); }
+// tag of a live key, 2..255: bits 16..31 of the key hash, which no capacity's home slot uses, reduced to 254 values
+enum : uint8_t { TAG_EMPTY = 0, TAG_TOMB = 1 };
+__host__ __device__ inline uint8_t tag_of(uint32_t pos, uint64_t content) {
+    return (uint8_t)(2u + ((((uint32_t)key_hash(pos, content) >> 16) * 254u) >> 16));
+}
+__host__ __device__ inline uint8_t slot_tag(uint32_t state, uint32_t pos, uint64_t content) {
+    return state == SLOT_EMPTY ? (uint8_t)TAG_EMPTY : state == SLOT_TOMB ? (uint8_t)TAG_TOMB : tag_of(pos, content);
 }
 
 struct BlockRec { uint32_t pos; uint64_t content; uint64_t prefix; };
@@ -125,7 +142,7 @@ private:
     uint64_t workers_version_ = 0;
 
     // device mirror
-    DevBuf d_slots_, d_rows_, d_multi_, d_tree_;
+    DevBuf d_slots_, d_rows_, d_multi_, d_tree_, d_tags_;
     PinBuf stage_;
     DevBuf d_stage_;
     cudaEvent_t stage_done_ = nullptr;

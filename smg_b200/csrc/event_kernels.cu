@@ -73,17 +73,82 @@ __device__ __forceinline__ MultiNode load_node(const MultiNode* p) {
     return n;
 }
 
-// DashMap::get(&(position, content_hash)) — linear probing over 32 B slots.  Works per-thread (divergent) or
-// warp-uniform (same address in every lane → one broadcast transaction).
-__device__ __forceinline__ bool probe(const EventIndexView& v, uint32_t pos, uint64_t content, Slot& out) {
-    uint32_t h = slot_hash(pos, content) & v.mask;
+// 16 B of the tag array, kept in L2 (evict-last): the tags are 1/32 of the slots' size and are read by every chain walk
+__device__ __forceinline__ uint4 ld_tags(const uint8_t* p) {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    uint4 r;
+    asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol));
+    return r;
+}
+// bit k set ⟺ byte k of the 16 B word equals the byte replicated in `rep`
+__device__ __forceinline__ uint32_t byte_eq_bits(const uint4 w, uint32_t rep) {
+    auto four = [&](uint32_t x) { return ((__vcmpeq4(x, rep) & 0x01010101u) * 0x01020408u) >> 24; };   // bytes 0..3 → bits 0..3
+    return four(w.x) | (four(w.y) << 4) | (four(w.z) << 8) | (four(w.w) << 12);
+}
+
+// DashMap::get(&(position, content_hash)) from slot h on, walked in the tag bytes: the aligned 32 B tag sector holding h is read, the
+// chain is followed there up to its first empty tag (the next sector only when the chain runs past this one's end, wrapping at the
+// mask), and a 32 B slot is loaded only where the tag equals the key's; its full key is then compared, so a tag collision costs one
+// slot read and never a wrong answer.  Per-thread (divergent).  The walk is split in three steps so that a caller with two lookups can
+// have both tag loads, then both slot loads in flight together: tag_sector, the load of tag_slot, tag_finish.
+__device__ __forceinline__ uint32_t tag_rep(uint32_t pos, uint64_t content) { return (uint32_t)tag_of(pos, content) * 0x01010101u; }
+struct TagCursor { uint32_t base, cand; bool ends; };   // one tag sector: the candidate slots left in it, and whether the chain ends in it
+__device__ __forceinline__ TagCursor tag_sector(const EventIndexView& v, uint32_t rep, uint32_t h) {
+    const uint32_t base = h & ~31u;   // capacity ≥ 1024: a sector never straddles the end of the table
+    const uint4 t0 = ld_tags(v.tags + base), t1 = ld_tags(v.tags + base + 16);
+    const uint32_t from = ~0u << (h & 31u);
+    const uint32_t empty = (byte_eq_bits(t0, 0u) | (byte_eq_bits(t1, 0u) << 16)) & from;
+    uint32_t cand = (byte_eq_bits(t0, rep) | (byte_eq_bits(t1, rep) << 16)) & from;
+    if (empty) cand &= (empty & (0u - empty)) - 1u;   // only the slots before the first empty one
+    return TagCursor{base, cand, empty != 0};
+}
+__device__ __forceinline__ uint32_t tag_slot(const TagCursor& c) { return c.base + (uint32_t)(__ffs((int)c.cand) - 1); }
+__device__ __forceinline__ bool key_is(const Slot& s, uint32_t pos, uint64_t content) {
+    return s.state != SLOT_EMPTY && s.state != SLOT_TOMB && s.content == content && s.pos == pos;
+}
+// `s` is slot tag_slot(c) when c.cand is non-zero (loaded by the caller)
+__device__ __forceinline__ bool tag_finish(const EventIndexView& v, uint32_t pos, uint64_t content, uint32_t rep, TagCursor c, Slot s, Slot& out) {
 #pragma unroll 1
     for (;;) {
-        Slot s = load_slot(v.slots + h);
-        if (s.state == SLOT_EMPTY) return false;
-        if (s.state != SLOT_TOMB && s.content == content && s.pos == pos) { out = s; return true; }
-        h = (h + 1) & v.mask;
+        while (c.cand) {
+            if (key_is(s, pos, content)) { out = s; return true; }
+            c.cand &= c.cand - 1u;
+            if (c.cand) s = load_slot(v.slots + tag_slot(c));
+        }
+        if (c.ends) return false;
+        c = tag_sector(v, rep, (c.base + 32u) & v.mask);
+        if (c.cand) s = load_slot(v.slots + tag_slot(c));
     }
+}
+__device__ __forceinline__ bool tag_walk(const EventIndexView& v, uint32_t pos, uint64_t content, uint32_t h, Slot& out) {
+    const uint32_t rep = tag_rep(pos, content);
+    const TagCursor c = tag_sector(v, rep, h);
+    Slot s{0, 0, SLOT_EMPTY, 0, 0};
+    if (c.cand) s = load_slot(v.slots + tag_slot(c));
+    return tag_finish(v, pos, content, rep, c, s, out);
+}
+// The same lookup from the key's home slot: no slot is read for an absent key unless its tag collides.
+__device__ __forceinline__ bool tag_probe(const EventIndexView& v, uint32_t pos, uint64_t content, Slot& out) {
+    return tag_walk(v, pos, content, slot_hash(pos, content) & v.mask, out);
+}
+// The rest of a lookup whose home slot h has been read into s: done when s is empty or is the key, else the chain goes on in the tags.
+__device__ __forceinline__ bool finish_probe(const EventIndexView& v, uint32_t pos, uint64_t content, uint32_t h, Slot& s) {
+    if (s.state == SLOT_EMPTY) return false;
+    if (s.state != SLOT_TOMB && s.content == content && s.pos == pos) return true;
+    if (tag_walk(v, pos, content, (h + 1) & v.mask, s)) return true;
+    s.state = SLOT_EMPTY;   // as a walk over the slots would have left it: the empty slot that ended the chain
+    return false;
+}
+
+// DashMap::get(&(position, content_hash)) — the home slot first (hot entries are L2 hits), the collision chain in the tags.  Works
+// per-thread (divergent) or warp-uniform (same address in every lane → one broadcast transaction).
+__device__ __forceinline__ bool probe(const EventIndexView& v, uint32_t pos, uint64_t content, Slot& out) {
+    const uint32_t h = slot_hash(pos, content) & v.mask;
+    Slot s = load_slot(v.slots + h);
+    if (!finish_probe(v, pos, content, h, s)) return false;
+    out = s;
+    return true;
 }
 
 // ---- worker sets --------------------------------------------------------------------------------------------
@@ -361,15 +426,6 @@ __device__ __forceinline__ void write_pick(const BatchDesc& b, uint32_t r, int32
 // independent slot loads up front (position 0 and the first jump destination), the count test, and only on a
 // failed test the linear drain (4 probes in flight at a time).  ~30 warp-instructions per request on the common
 // path; the kernel is a few microseconds for 10^5 requests and disappears next to the hash stream.
-__device__ __forceinline__ bool finish_probe(const EventIndexView& v, uint32_t pos, uint64_t content, uint32_t h, Slot& s) {
-#pragma unroll 1
-    for (;;) {
-        if (s.state == SLOT_EMPTY) return false;
-        if (s.state != SLOT_TOMB && s.content == content && s.pos == pos) return true;
-        h = (h + 1) & v.mask;
-        s = load_slot(v.slots + h);
-    }
-}
 __device__ __forceinline__ bool t_entry_set(const EventIndexView& v, const Slot& s, const uint64_t* ch, int p, PrefixCache& pc, uint64_t& set) {
     if (s.state == SLOT_SINGLE) { set = s.payload; return true; }
     uint64_t want = prefix_at(ch, p, pc);
@@ -1538,10 +1594,10 @@ __global__ void __launch_bounds__(128, MINB) event_tile_kernel(const __grid_cons
 //   A  one THREAD per request: offsets, the fleet gate, the tokens of blocks 0 and last (all eight 16 B loads issued before either hash),
 //      both hashes, both probes in flight together, the count-only jump test (event_tree.rs:720).  A block's content hash depends on
 //      that block alone, so a full hit or a novel request reads 128 B of tokens.  A failed count test goes onto a shared-memory queue
-//      together with both hashes;
-//   B  the queue is striped over the CTA's 8 warps, two drains per round so that the loads and probes of the second overlap those of
-//      the first: lane p (1 ≤ p < last) reads and hashes block p, lanes 0 and last take the queued hashes, every position is probed at
-//      once and drain_resolve replays the ordered scan.
+//      together with what both probes found;
+//   B  the queue is striped over the CTA's 8 warps, two drains per round so that the loads and lookups of the second overlap those of
+//      the first: lane p (1 ≤ p < last) reads and hashes block p and looks it up in the tag array (tag_sector / tag_finish: a slot is
+//      read only where the tag matches), lanes 0 and last take the queued probes, and drain_resolve replays the ordered scan.
 // What needs the rolling prefix hashes or more than one jump (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device
 // queue, at most once per request (from A or from B), and finished by event_slow_kernel right behind.
 struct SimpleLoc { uint32_t j, r; };
@@ -1552,7 +1608,7 @@ __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t 
     return l;
 }
 
-struct LaneDrain { uint32_t g, off, ntok, pad; uint64_t c0, c1; };   // a failed count test: request, token range, hashes of blocks 0 and last
+struct LaneDrain { uint32_t g, off, ntok, f1; uint64_t p0, p1; };   // a failed count test: request, token range, the probes of blocks 0 and last
 
 __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
                                                             uint32_t* __restrict__ slow_queue) {
@@ -1599,7 +1655,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
                 if (f1 && s1.state != SLOT_SINGLE) to_slow(g);
                 else if (f1 && __popcll(s1.payload) == __popcll(s0.payload))   // count-only jump test (:720)
                     finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, s0.payload & elig, nb, ntok);
-                else s_q[atomicAdd(&s_n, 1u)] = LaneDrain{g, off, ntok, 0, c0, c1};
+                else s_q[atomicAdd(&s_n, 1u)] = LaneDrain{g, off, ntok, (uint32_t)f1, s0.payload, s1.payload};
             }
         }
     }
@@ -1619,20 +1675,30 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
         const LaneDrain& d1 = s_q[two ? q + 8 : q];
         const int last0 = (int)(d0.ntok >> 4) - 1, last1 = two ? (int)(d1.ntok >> 4) - 1 : -1;   // last1 = -1: no second drain this round
         const bool m0 = lane >= 1 && lane < last0, m1 = lane >= 1 && lane < last1;
+        // the second block is prefetched into L2 and loaded once the first is hashed: both blocks in registers at once leave too few
+        // for the lookups below (spills at 64 registers)
+        const uint32_t* p1 = m1 ? a.b[simple_locate(a, d1.g).j].tokens + d1.off + (size_t)lane * 16 : nullptr;
+        if (m1) asm volatile("prefetch.global.L2 [%0];\n\tprefetch.global.L2 [%1];" ::"l"(p1), "l"(p1 + 8));
         uint32_t w0[16], w1[16];
-        if (m0) load_block16(a.b[simple_locate(a, d0.g).j].tokens + d0.off + (size_t)lane * 16, w0);
-        if (m1) load_block16(a.b[simple_locate(a, d1.g).j].tokens + d1.off + (size_t)lane * 16, w1);
-        uint64_t h0 = lane == 0 ? d0.c0 : d0.c1, h1 = lane == 0 ? d1.c0 : d1.c1;
-        if (m0) h0 = xxh3_16words(w0, kSeed);
-        if (m1) h1 = xxh3_16words(w1, kSeed);
-        // every position of both requests probed at once (0 and last again: L2-hot)
-        const uint32_t i0 = slot_hash((uint32_t)lane, h0) & v.mask, i1 = slot_hash((uint32_t)lane, h1) & v.mask;
+        uint64_t h0 = 0, h1 = 0;
+        if (m0) { load_block16(a.b[simple_locate(a, d0.g).j].tokens + d0.off + (size_t)lane * 16, w0); h0 = xxh3_16words(w0, kSeed); }
+        if (m1) { load_block16(p1, w1); h1 = xxh3_16words(w1, kSeed); }
+        // positions 1..last-1 of both requests looked up at once in the tags (both tag loads, then both slot loads in flight); about
+        // half of them are absent keys, which then read no slot.  Positions 0 and last are phase A's probes, carried in the queue.
+        const uint32_t rep0 = tag_rep((uint32_t)lane, h0), rep1 = tag_rep((uint32_t)lane, h1);
+        TagCursor c0{0, 0, true}, c1{0, 0, true};
+        if (m0) c0 = tag_sector(v, rep0, slot_hash((uint32_t)lane, h0) & v.mask);
+        if (m1) c1 = tag_sector(v, rep1, slot_hash((uint32_t)lane, h1) & v.mask);
         Slot sl0{0, 0, SLOT_EMPTY, 0, 0}, sl1{0, 0, SLOT_EMPTY, 0, 0};
-        if (lane <= last0) sl0 = load_slot(v.slots + i0);
-        if (lane <= last1) sl1 = load_slot(v.slots + i1);
+        if (c0.cand) sl0 = load_slot(v.slots + tag_slot(c0));
+        if (c1.cand) sl1 = load_slot(v.slots + tag_slot(c1));
         bool f0 = false, f1 = false;
-        if (lane <= last0) f0 = finish_probe(v, (uint32_t)lane, h0, i0, sl0);
-        if (lane <= last1) f1 = finish_probe(v, (uint32_t)lane, h1, i1, sl1);
+        if (m0) f0 = tag_finish(v, (uint32_t)lane, h0, rep0, c0, sl0, sl0);
+        if (m1) f1 = tag_finish(v, (uint32_t)lane, h1, rep1, c1, sl1, sl1);
+        __syncwarp();   // keeps the queued probes' shared-memory loads here: hoisted above the token loads they cost the registers of a spill
+        if (lane == 0) { f0 = true; sl0.state = SLOT_SINGLE; sl0.payload = d0.p0; f1 = true; sl1.state = SLOT_SINGLE; sl1.payload = d1.p0; }
+        if (lane == last0) { f0 = d0.f1 != 0; sl0.state = SLOT_SINGLE; sl0.payload = d0.p1; }
+        if (lane == last1) { f1 = d1.f1 != 0; sl1.state = SLOT_SINGLE; sl1.payload = d1.p1; }
         const DrainResult r0 = drain_resolve(last0 + 1, elig, lane, f0, sl0);
         if (lane == 0) drain_done(d0, r0);
         if (two) {
@@ -1645,7 +1711,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
 // The same pick with one WARP per request, for launches too small to give every SM a CTA of event_lane_kernel (a lone batch of a few
 // thousand requests): ⌈requests / 8⌉ CTAs spread the work over all SMs, where the lane kernel's ⌈requests / 256⌉ would occupy a few.
 // Lane p owns block p; lanes 0 and last hash their blocks and probe the two jump destinations, and only a failed count test makes lanes
-// 1..last-1 read and hash theirs for drain_resolve.  Rare shapes go to the same queue for event_slow_kernel.
+// 1..last-1 read and hash theirs and look them up in the tag array for drain_resolve.  Rare shapes go to the same queue for event_slow_kernel.
 __global__ void __launch_bounds__(256, 5) event_warp_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
                                                             uint32_t* __restrict__ slow_queue) {
     __shared__ int32_t s_slice[64];
@@ -1697,7 +1763,7 @@ __global__ void __launch_bounds__(256, 5) event_warp_kernel(const __grid_constan
                             uint32_t count = 0;   // count_workers_at(last) (:555-574)
                             if (fl) { if (stl == SLOT_SINGLE) count = (uint32_t)__popcll(shfl64(sl.payload, last)); else bail = true; }
                             if (!bail && count != (uint32_t)__popcll(active)) {
-                                if (lane >= 1 && lane < last) found = probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
+                                if (lane >= 1 && lane < last) found = tag_probe(v, (uint32_t)lane, hash_block<16>(b.tokens + off + (size_t)lane * 16, 16), sl);
                                 const DrainResult d = drain_resolve((int)nb, elig, lane, found, sl);
                                 bail = d.bail; win = d.win; score = d.score;
                             }
