@@ -193,6 +193,7 @@ void EventIndex::insert_entry(uint32_t pos, uint64_t content, uint64_t prefix, u
         uint32_t b = new_multi(prefix, nset, a);
         Slot& s2 = slots_[(size_t)f];  // new_set may have grown rows_, never slots_
         s2.state = SLOT_MULTI;
+        ++multi_slots_;
         s2.prefix = 0;
         s2.payload = b;
         mark_slot((uint32_t)f);
@@ -242,6 +243,7 @@ void EventIndex::drop_entry(const BlockRec& r, uint32_t wid) {
         now_empty = (uint32_t)s.payload == kNil;
     }
     if (now_empty) {
+        if (s.state == SLOT_MULTI) --multi_slots_;
         s.state = SLOT_TOMB;
         s.payload = 0;
         --live_;
@@ -327,6 +329,7 @@ void EventIndex::rebuild(uint32_t new_capacity, uint32_t new_words) {
     mask_ = new_capacity - 1;
     live_ = 0;
     tombs_ = 0;
+    multi_slots_ = 0;
     full_dirty_ = true;
     dirty_slots_.clear(); dirty_multi_.clear(); dirty_rows_.clear();
 
@@ -346,6 +349,7 @@ void EventIndex::rebuild(uint32_t new_capacity, uint32_t new_words) {
         Slot& s = slots_[h];
         s.content = o.content; s.pos = o.pos; s.state = o.state; s.prefix = o.prefix;
         if (o.state == SLOT_SINGLE) { s.payload = convert(o.payload); continue; }
+        ++multi_slots_;
         uint32_t head = kNil;
         for (uint32_t i = (uint32_t)o.payload; i != kNil; i = old_multi[i].next) {
             uint32_t ni = (uint32_t)multi_.size();

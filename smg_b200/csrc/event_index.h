@@ -97,6 +97,8 @@ public:
     void remove_worker(uint32_t wid);
     uint64_t current_size() const;                                        // :438-444
     uint64_t entry_count() const { return live_; }
+    // slots in state MULTI: while there is none, no lookup can need a rolling prefix hash
+    uint64_t multi_count() const { return multi_slots_; }
     uint32_t n_workers() const { return (uint32_t)tree_sizes_.size(); }
     uint32_t jump() const { return jump_; }
     uint64_t workers_version() const { return workers_version_; }
@@ -131,7 +133,7 @@ private:
     uint32_t words_ = 1;
     std::vector<Slot> slots_;
     uint32_t mask_ = 0;
-    uint64_t live_ = 0, tombs_ = 0;
+    uint64_t live_ = 0, tombs_ = 0, multi_slots_ = 0;
     std::vector<uint64_t> rows_;
     std::vector<uint32_t> free_rows_;
     std::vector<MultiNode> multi_;

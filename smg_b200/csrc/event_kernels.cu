@@ -1599,7 +1599,8 @@ __global__ void __launch_bounds__(128, MINB) event_tile_kernel(const __grid_cons
 //      the first: lane p (1 ≤ p < last) reads and hashes block p and looks it up in the tag array (tag_sector / tag_finish: a slot is
 //      read only where the tag matches), lanes 0 and last take the queued probes, and drain_resolve replays the ordered scan.
 // What needs the rolling prefix hashes or more than one jump (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device
-// queue, at most once per request (from A or from B), and finished by event_slow_kernel right behind.
+// queue, at most once per request (from A or from B), and finished by event_slow_kernel right behind.  That kernel is launched only when
+// such a request is possible: the index holds a Multi entry, or the launch allows more than 32 blocks or more than one jump (MultiArgs.skip_slow).
 struct SimpleLoc { uint32_t j, r; };
 __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t g) {
     SimpleLoc l;
@@ -1609,6 +1610,13 @@ __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t 
 }
 
 struct LaneDrain { uint32_t g, off, ntok, f1; uint64_t p0, p1; };   // a failed count test: request, token range, the probes of blocks 0 and last
+
+// queues request g for event_slow_kernel; a launch that skipped that kernel (a.skip_slow) reports it as an internal error instead (a bit
+// OR-ed into err_flag, as the over-the-cap 1 of these kernels is, so that neither clears the other)
+__device__ __forceinline__ void push_slow(const MultiArgs& a, uint32_t* slow_queue, uint32_t g) {
+    if (a.skip_slow) atomicOr(a.err_flag, kErrNoSlowKernel);
+    else slow_queue[2 + atomicAdd(slow_queue, 1u)] = g;
+}
 
 __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constant__ EventIndexView v, FleetView f, const __grid_constant__ MultiArgs a,
                                                             uint32_t* __restrict__ slow_queue) {
@@ -1626,7 +1634,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
     __syncthreads();
     const int32_t min_load_idx = f.derived->min_load_idx;
     const uint64_t elig = f.elig[0];
-    auto to_slow = [&](uint32_t g) { slow_queue[2 + atomicAdd(slow_queue, 1u)] = g; };
+    auto to_slow = [&](uint32_t g) { push_slow(a, slow_queue, g); };
 
     // ---- phase A ----
     const uint32_t g = blockIdx.x * 256 + threadIdx.x;
@@ -1637,7 +1645,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
         const uint32_t nb = ntok >> 4;
         if (f.derived->n_healthy == 0) write_pick(b, loc.r, -1, SMGX_BR_NO_HEALTHY, 0, ntok);
         else if (f.derived->imbalanced) write_pick(b, loc.r, min_load_idx, SMGX_BR_IMBALANCED_MIN_LOAD, 0, ntok);
-        else if (nb > a.max_blocks) { atomicExch(a.err_flag, 1u); write_pick(b, loc.r, -1, 255, 0, ntok); }
+        else if (nb > a.max_blocks) { atomicOr(a.err_flag, 1u); write_pick(b, loc.r, -1, 255, 0, ntok); }
         else if (nb == 0 || v.n_workers == 0) finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, 0, 0, ntok);
         else if (nb > 32 || nb - 1 > v.jump) to_slow(g);   // more than one jump / more blocks than lanes: the generic search
         else {
@@ -1736,12 +1744,12 @@ __global__ void __launch_bounds__(256, 5) event_warp_kernel(const __grid_constan
     } else if (fd->imbalanced) { out = fd->min_load_idx; branch = SMGX_BR_IMBALANCED_MIN_LOAD; }
     else {
         const uint32_t nb = ntok >> 4;
-        if (nb > a.max_blocks) { if (lane == 0) atomicExch(a.err_flag, 1u); branch = 255; }
+        if (nb > a.max_blocks) { if (lane == 0) atomicOr(a.err_flag, 1u); branch = 255; }
         else {
             out = fd->min_load_idx; branch = SMGX_BR_EVENT_MIN_LOAD;   // until an overlap is found
             if (nb > 0 && v.n_workers > 0) {
                 if (nb > 32 || nb - 1 > v.jump) {   // more than one jump / more blocks than lanes: the generic search
-                    if (lane == 0) slow_queue[2 + atomicAdd(slow_queue, 1u)] = g;
+                    if (lane == 0) push_slow(a, slow_queue, g);
                     return;
                 }
                 const int last = (int)nb - 1;
@@ -1771,7 +1779,7 @@ __global__ void __launch_bounds__(256, 5) event_warp_kernel(const __grid_constan
                     }
                 }
                 if (bail) {
-                    if (lane == 0) slow_queue[2 + atomicAdd(slow_queue, 1u)] = g;
+                    if (lane == 0) push_slow(a, slow_queue, g);
                     return;
                 }
                 if (win) {
@@ -2180,18 +2188,21 @@ static bool event_lane_selected() {   // SMGX_EVENT_SIMPLE=0|4|5|6: 0 = do not u
     }
     return v != 0;
 }
-static void launch_lane(const EventIndexView& ix, const FleetView& fleet, const MultiArgs& a, int sm_count, cudaStream_t stream, uint32_t* d_queue) {
+// → the number of kernels launched: 1 when a.skip_slow (event_slow_kernel could get no request), else 2
+static int launch_lane(const EventIndexView& ix, const FleetView& fleet, const MultiArgs& a, int sm_count, cudaStream_t stream, uint32_t* d_queue) {
     // one thread per request once the launch gives every SM a CTA of 256; below that (a lone batch of a few thousand requests) one warp per
     // request spreads the work over all SMs and answers sooner (measured on H100: 4096 requests, §5 of DESIGN.md)
     if (a.total >= 256u * (unsigned)sm_count) event_lane_kernel<<<(a.total + 255) / 256, 256, 0, stream>>>(ix, fleet, a, d_queue);
     else event_warp_kernel<<<(a.total + 7) / 8, 256, 0, stream>>>(ix, fleet, a, d_queue);
     SMGX_CUDA(cudaGetLastError());
+    if (a.skip_slow) return 1;
     const size_t smem = (size_t)std::max<uint32_t>(a.max_blocks, 1) * 8 * 8;
     if (smem > 48 * 1024) SMGX_CUDA(cudaFuncSetAttribute(event_slow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // one warp per queued request: ⌈total / 8⌉ CTAs would give every request a warp, two per SM are plenty for the rare shapes it gets
     const unsigned slow_grid = std::min<unsigned>((unsigned)sm_count * 2, std::max(1u, (a.total + 7) / 8));
     event_slow_kernel<<<slow_grid, 256, smem, stream>>>(ix, fleet, a, d_queue);
     SMGX_CUDA(cudaGetLastError());
+    return 2;
 }
 
 static std::atomic<int> g_tile_depth{-1};
@@ -2371,8 +2382,7 @@ void launch_event_select(const EventIndexView& ix, const FleetView& fleet, const
             bool plain = true;
             for (uint32_t j = 0; j < a.count; ++j) plain = plain && a.b[j].cand == nullptr;
             if (plain) {
-                launch_lane(ix, fleet, a, sm_count, stream, a.slow_queue);
-                *launches += 2;
+                *launches += launch_lane(ix, fleet, a, sm_count, stream, a.slow_queue);
                 return;
             }
         }

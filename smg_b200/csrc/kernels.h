@@ -50,6 +50,8 @@ void launch_fleet_prepare(const FleetRaw& raw, FleetDerived* d_derived, int32_t*
 //                                (one thread per request for fleets ≤ 64 interned workers, one warp per request above)
 //   `hashes` is then a scratch of sum(n) × max_blocks u64 laid out [request][max_blocks], written and read back out of L2.
 constexpr int kMaxMultiBatches = 32;
+// MultiArgs.err_flag bit (OR-ed in): a request needed event_slow_kernel in a launch that skipped it (MultiArgs.skip_slow); its pick is not written
+constexpr uint32_t kErrNoSlowKernel = 4;
 // what the hash kernel leaves per request for the search kernel's first phase: the two hashes the jump search probes first and the
 // request's length — one 32 B record instead of the chain offsets → hash row → slots
 struct alignas(32) SearchRec { uint64_t h0, h1; uint32_t ntok, pad0; uint64_t pad1; };
@@ -86,6 +88,9 @@ struct MultiArgs {
     const void* pf_slots;          // EventIndexView.slots (nullable)
     uint32_t pf_mask, pf_jump;
     uint32_t* slow_queue;          // event_lane_kernel / event_warp_kernel → event_slow_kernel: [0] = count, [1] = CTA exit counter (both zero between launches), [2 .. total + 1] = request indices (each request pushed at most once)
+    // 1: no request of this launch can be queued for event_slow_kernel (the index view holds no Multi entry, max_blocks ≤ 32 and
+    // max_blocks − 1 ≤ jump), so it is not launched; a request that still reaches the queue sets err_flag to kErrNoSlowKernel
+    uint32_t skip_slow;
     uint64_t* fb_winsets;
     uint32_t* fb_scores;           // 0xFFFFFFFF = request longer than max_blocks
     // one-launch path (event_hs_kernel): per (batch, group of 256 requests) arrival counters, zero between launches

@@ -310,6 +310,9 @@ public:
                 SMGX_CUDA(cudaMemsetAsync(lane.d_slowq.ptr, 0, lane.d_slowq.cap, lane.stream));
             }
             a.slow_queue = lane.d_slowq.as<uint32_t>();
+            // a request is queued for event_slow_kernel only when it has more than 32 blocks, more than one jump, or meets a Multi entry:
+            // with none of these possible (the multi count is the one of the view sync_state just flushed) the kernel is not launched
+            a.skip_slow = m.indexer->multi_count() == 0 && a.max_blocks <= 32 && a.max_blocks - 1 <= ixv.jump;
         }
         a.fb_winsets = nullptr; a.fb_scores = nullptr;
         const bool feedback = load_feedback && !cand_mode && rows > 0;
@@ -1862,6 +1865,10 @@ static smgx_status select_batch_text_once(smgx_policy* p, const char* model_key,
         if (may_overflow) {   // a request over max_tokens_per_request only after normalization: reported by this call, once
             uint32_t flag = 0;
             SMGX_CUDA(cudaMemcpy(&flag, P.d_err.ptr, 4, cudaMemcpyDeviceToHost));
+            if (flag & kErrNoSlowKernel) {
+                SMGX_CUDA(cudaMemset(P.d_err.ptr, 0, 4));
+                throw Error(SMGX_UNKNOWN_ERROR, "internal error: a request needed event_slow_kernel in a launch that did not run it");
+            }
             if (flag == 1) {
                 SMGX_CUDA(cudaMemset(P.d_err.ptr, 0, 4));
                 throw Error(SMGX_INVALID_ARGUMENT, "a request exceeded max_tokens_per_request after normalization");
@@ -2769,6 +2776,8 @@ smgx_status smgx_synchronize(smgx_policy* p, char** err) {
         SMGX_CUDA(cudaMemcpy(&flag, p->impl.d_err.ptr, 4, cudaMemcpyDeviceToHost));
         if (flag) {
             SMGX_CUDA(cudaMemset(p->impl.d_err.ptr, 0, 4));
+            if (flag & kErrNoSlowKernel)   // OR-ed into the flag (the lane and warp kernels OR their over-the-cap 1 as well), checked first
+                throw Error(SMGX_UNKNOWN_ERROR, "internal error: a request needed event_slow_kernel in a launch that did not run it");
             if (flag == 2) throw Error(SMGX_DEVICE_ERROR, "peer-memory exchange: a rank did not publish its candidates in time");
             if (flag == 3) throw Error(SMGX_DEVICE_ERROR, "concurrent split launch: the search kernel gave up waiting for the hash kernel");
             throw Error(SMGX_INVALID_ARGUMENT, "a request exceeded max_tokens_per_request on the device-resident path");
