@@ -632,10 +632,11 @@ StrSlot StringTreeIndex::device_slot(uint32_t i) const {
 StringTreeView StringTreeIndex::flush(cudaStream_t stream, uint64_t* launches) {
     if (!device_enabled) throw Error(SMGX_DEVICE_ERROR, "policy was created with device_id = -1 (host mirror only): no GPU path, no CPU fallback");
     if (tenants_version_seen != tenants_->version) { full_dirty_ = true; tenants_version_seen = tenants_->version; }
-    if (bytes_.size() + 16 > d_bytes_.cap) {
+    // 32 B of slack past the arena: load16_global reads the aligned 16 B chunk after the one holding a label's last byte
+    if (bytes_.size() + 32 > d_bytes_.cap) {
         if (stage_pending_) { SMGX_CUDA(cudaEventSynchronize(stage_done_)); stage_pending_ = false; }
         SMGX_CUDA(cudaDeviceSynchronize());
-        d_bytes_.reserve(std::max<size_t>(bytes_.capacity() * 2, 4096) + 16);
+        d_bytes_.reserve(std::max<size_t>(bytes_.capacity() * 2, 4096) + 32);
         uploaded_bytes_ = 0;
     }
     if (uploaded_bytes_ < bytes_.size()) {
@@ -709,7 +710,10 @@ __device__ __forceinline__ uint4 load16_global(const uint8_t* p) {
     if (s == 0) return lo;
     return shift16(lo, __ldg(a + 1), s);
 }
-__device__ __forceinline__ uint4 load16_shared(const uint8_t* p) {   // p inside a 16-byte-aligned shared array with 16 bytes of slack
+// Both loads read the aligned 16-byte chunk holding p and, when p is unaligned, the next one: up to 30 bytes past p.  A lane whose
+// 16 bytes start at a label's last byte therefore reads up to 30 bytes past the label's end — the label arena keeps 32 bytes of slack
+// past its end (StringTreeIndex::flush), the staging window 32 bytes past kTxtWin.
+__device__ __forceinline__ uint4 load16_shared(const uint8_t* p) {
     const uint32_t s = (uint32_t)(__cvta_generic_to_shared(p) & 15);
     const uint4* a = reinterpret_cast<const uint4*>(p - s);
     const uint4 lo = a[0];
