@@ -335,9 +335,13 @@ smgx_status smgx_select_batch_request_text(smgx_policy* p, const char* model_key
  *   SMGX_PRETOK_CL100K  CL100K_BASE_PATTERN (tiktoken.rs:28): cl100k_base, and the Llama-3 Split regex of tokenizer.json files;
  *   SMGX_PRETOK_R50K    tiktoken's GPT-2 pattern r50k_pat_str: r50k_base, p50k_base, p50k_edit, and tokenizer.json files whose
  *                       pre-tokenizer is ByteLevel(use_regex = true, add_prefix_space = false) alone;
- *   SMGX_PRETOK_QWEN2   the Qwen2 Split regex: the cl100k pattern with \p{N} in place of \p{N}{1,3} (every digit is a piece).
- * Any other value is SMGX_INVALID_ARGUMENT. */
-typedef enum smgx_pretokenizer { SMGX_PRETOK_CL100K = 0, SMGX_PRETOK_R50K = 1, SMGX_PRETOK_QWEN2 = 2 } smgx_pretokenizer;
+ *   SMGX_PRETOK_QWEN2   the Qwen2 Split regex: the cl100k pattern with \p{N} in place of \p{N}{1,3} (every digit is a piece);
+ *   SMGX_PRETOK_DEEPSEEK  the chain of three Isolated Splits of DeepSeek V2 / V2.5 / Coder-V2 / V3 / V3.1 / R1 tokenizer.json files:
+ *                       \p{N}{1,3}, then kana/CJK runs [一-龥぀-ゟ゠-ヿ]+, then the DeepSeek word regex on every piece (bpe.cuh).
+ * Any other value (3 included) is SMGX_INVALID_ARGUMENT. */
+typedef enum smgx_pretokenizer {
+    SMGX_PRETOK_CL100K = 0, SMGX_PRETOK_R50K = 1, SMGX_PRETOK_QWEN2 = 2, SMGX_PRETOK_DEEPSEEK = 4
+} smgx_pretokenizer;
 /* The tokenizer.json normalizer applied to the text between special tokens before it is split:
  *   SMGX_NORMALIZER_NONE  none;
  *   SMGX_NORMALIZER_NFC   {"type": "NFC"} (Qwen2 and later), with the Unicode tables of the `tokenizers` crate.
@@ -361,7 +365,9 @@ smgx_status smgx_tokenizer_load_tiktoken_ex(smgx_policy* p, const char* model_ke
                                             const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err);
 /* HuggingFaceTokenizer (crates/tokenizer/src/huggingface.rs:310-316 → crate `tokenizers`), byte-level BPE family whose tokenizer.json
  * has: no normalizer; pre_tokenizer = Split(Regex = the cl100k pattern above, Isolated) + ByteLevel(use_regex = false) — Llama 3 and
- * kin — or, with SMGX_PRETOK_R50K through the _ex form, ByteLevel(use_regex = true, add_prefix_space = false) alone — GPT-2 and kin;
+ * kin — or, with SMGX_PRETOK_R50K through the _ex form, ByteLevel(use_regex = true, add_prefix_space = false) alone — GPT-2 and kin,
+ * or, with SMGX_PRETOK_DEEPSEEK, DeepSeek's Sequence of three Splits + ByteLevel(use_regex = false) (its empty-Sequence normalizer is
+ * the identity: load it with SMGX_NORMALIZER_NONE);
  * model.type = "BPE" without dropout / unk / byte_fallback.  The caller parses the JSON (serde_json in the gateway,
  * smg_b200/policy.py here) and hands over: token i = blob[tok_offsets[i] .. tok_offsets[i+1]) as RAW bytes (byte-level chars mapped
  * back) with id ids[i]; `merges` = n_merges (left id, right id) pairs in priority order; model.ignore_merges; added_tokens as specials. */

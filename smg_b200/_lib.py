@@ -10,7 +10,7 @@ HEADER = os.path.join(os.path.dirname(HERE), "include", "smgx.h")
 
 SUCCESS, INVALID_ARGUMENT, TOKENIZATION_ERROR, MEMORY_ERROR, DEVICE_ERROR = 0, 1, 2, 4, 5
 WORKER_NOT_TRACKED, PARENT_BLOCK_NOT_FOUND, NOT_FOUND, BUSY, UNKNOWN_ERROR = 10, 11, 12, 13, 99
-PRETOK_CL100K, PRETOK_R50K, PRETOK_QWEN2 = 0, 1, 2   # smgx_pretokenizer
+PRETOK_CL100K, PRETOK_R50K, PRETOK_QWEN2, PRETOK_DEEPSEEK = 0, 1, 2, 4   # smgx_pretokenizer
 NORMALIZER_NONE, NORMALIZER_NFC = 0, 1   # smgx_normalizer
 SP_LEGACY, SP_METASPACE = 0, 1   # smgx_sp_shape
 PREPEND_NEVER, PREPEND_FIRST, PREPEND_ALWAYS = 0, 1, 2   # smgx_prepend_scheme

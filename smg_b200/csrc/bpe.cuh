@@ -165,7 +165,7 @@ SMGX_HD bool qwen2_anchor_rule(uint8_t pc, uint8_t c) { return (pc == CH_LETTER 
 //   's|'t|'re|'ve|'m|'ll|'d | ?\p{L}+ | ?\p{N}+ | ?[^\s\p{L}\p{N}]+ | \s+(?!\S) | \s+
 // Same contract as next_piece_cl100k.  Differences that matter: contractions are case-sensitive, digit runs are unbounded,
 // only U+0020 may lead a run, and there is no newline rule.
-enum class Pretok : uint8_t { Cl100k = 0, R50k = 1, Qwen2 = 2 };
+enum class Pretok : uint8_t { Cl100k = 0, R50k = 1, Qwen2 = 2, DeepSeek = 4 };
 
 SMGX_HD bool is_contraction_tail(uint8_t b) {   // second byte of 's 't 'm 'd 're 've 'll
     return b == 's' || b == 't' || b == 'm' || b == 'd' || b == 'r' || b == 'v' || b == 'l';
@@ -256,6 +256,129 @@ SMGX_HD bool is_anchor_qwen2(const uint8_t* s, uint32_t i, uint32_t beg, const u
     const uint8_t c = char_class(utf8_decode(s, i, i + 4, l), u);
     const uint8_t pc = char_class(prev_cp(s, i, beg), u);
     return qwen2_anchor_rule(pc, c);
+}
+
+// ---- DeepSeek pre-tokenizer ----------------------------------------------------------------------------------------
+// The tokenizer.json of DeepSeek V2 / V2.5 / Coder-V2 / V3 / V3.1 / R1 chains three Isolated Splits; each runs on every piece the one
+// before produced, a piece's end is the end of the string for the next regex, and unmatched gaps are pieces too:
+//   1. \p{N}{1,3}             digit runs, cut in triples counted from the start of the run
+//   2. [一-龥぀-ゟ゠-ヿ]+         kana/CJK runs (U+4E00-U+9FA5, U+3040-U+30FF); the generator asserts that no digit lies in them
+//   3. [!"#$%&'()*+,\-./:;<=>?@\[\\\]^_`{|}~][A-Za-z]+ | [^\r\n\p{L}\p{P}\p{S}]?[\p{L}\p{M}]+ | ?[\p{P}\p{S}]+[\r\n]* | \s*[\r\n]+ |
+//      \s+(?!\S) | \s+         on each kana/CJK run and on each stretch between digit and kana/CJK runs ("stage pieces")
+// The classes are those of `tokenizers` (Oniguruma), from deepseek_tables.h, not those of unicode_tables.h.
+enum : uint8_t { DS_OTHER = 0, DS_L = 1, DS_M = 2, DS_N = 3, DS_P = 4, DS_S = 5, DS_WS = 6, DS_KANA = 8 /* flag */ };
+constexpr uint8_t kDsEnd = 0xFF;
+
+SMGX_HD uint8_t ds_class(uint32_t cp, const UnicodeView& u) {   // u: the deepseek_tables.h ranges
+    if (cp < 0x80) {
+        if ((cp | 0x20) >= 'a' && (cp | 0x20) <= 'z') return DS_L;
+        if (cp >= '0' && cp <= '9') return DS_N;
+        if (cp == ' ' || (cp >= 0x09 && cp <= 0x0D)) return DS_WS;
+        if (cp == '$' || cp == '+' || (cp >= '<' && cp <= '>') || cp == '^' || cp == '`' || cp == '|' || cp == '~') return DS_S;
+        return cp >= 0x21 && cp <= 0x7E ? DS_P : DS_OTHER;
+    }
+    uint32_t a = 0, b = u.n;
+    while (a < b) {
+        uint32_t m = (a + b) >> 1;
+        if (u.hi[m] < cp) a = m + 1; else b = m;
+    }
+    return a < u.n && u.lo[a] <= cp ? u.cls[a] : (uint8_t)DS_OTHER;
+}
+SMGX_HD bool ds_letter_or_mark(uint8_t c) { return c == DS_L || c == DS_M; }   // c without the kana flag
+SMGX_HD bool ds_punct_or_symbol(uint8_t c) { return c == DS_P || c == DS_S; }
+SMGX_HD bool is_ascii_letter(uint8_t b) { return (b | 0x20) >= 'a' && (b | 0x20) <= 'z'; }
+// Class (kana flag dropped) of a character `c` (with its flag) seen from a stage piece of zone `z` (DS_KANA or 0), or kDsEnd when the
+// character ends that piece: a digit, or a character of the other zone.
+SMGX_HD uint8_t ds_stage_class(uint8_t c, uint8_t z) { return (c == DS_N || (c & DS_KANA) != z) ? kDsEnd : (uint8_t)(c & 7); }
+// ds_stage_class and length l of the character at byte j of s[0..n); kDsEnd at n and at a special's first byte (`stop` as in
+// next_piece_llama).
+SMGX_HD uint8_t ds_at(const uint8_t* s, uint32_t j, uint32_t n, const UnicodeView& u, const uint8_t* stop, uint8_t z, uint32_t& l) {
+    if (j >= n || (stop != nullptr && stop[j] == 2)) { l = 0; return kDsEnd; }
+    return ds_stage_class(ds_class(utf8_decode(s, j, n, l), u), z);
+}
+
+// Same contract as next_piece_cl100k, for the whole chain: i is a piece start (a digit at i starts a triple).
+SMGX_HD uint32_t next_piece_deepseek(const uint8_t* s, uint32_t i, uint32_t n, const UnicodeView& u, const uint8_t* stop = nullptr) {
+#define SMGX_AT_END(j) ((j) >= n || (stop != nullptr && stop[(j)] == 2))
+#define DS_AT(j, l) ds_at(s, (j), n, u, stop, c0 & DS_KANA, (l))
+    uint32_t len0;
+    const uint32_t cp0 = utf8_decode(s, i, n, len0);
+    const uint8_t c0 = ds_class(cp0, u);
+    uint32_t l;
+    // Split 1: \p{N}{1,3}
+    if (c0 == DS_N) {
+        uint32_t j = i + len0;
+        for (int c = 1; c < 3 && !SMGX_AT_END(j); ++c) {
+            if (ds_class(utf8_decode(s, j, n, l), u) != DS_N) break;
+            j += l;
+        }
+        return j;
+    }
+    // Split 3 inside the stage piece (kana/CJK run or the text between runs)
+    const uint8_t c = c0 & 7;
+    // 1. [ASCII punctuation][A-Za-z]+
+    if (cp0 < 0x80 && ds_punct_or_symbol(c)) {
+        uint32_t j = i + 1;
+        while (!SMGX_AT_END(j) && is_ascii_letter(s[j])) ++j;
+        if (j > i + 1) return j;
+    }
+    // 2. [^\r\n\p{L}\p{P}\p{S}]?[\p{L}\p{M}]+  — the optional char is taken only when a letter or mark follows it
+    {
+        uint32_t j = i;
+        bool ok = ds_letter_or_mark(c);
+        if (!ok && !ds_punct_or_symbol(c) && !is_newline(cp0) && ds_letter_or_mark(DS_AT(i + len0, l))) { j = i + len0; ok = true; }
+        if (ok) {
+            while (ds_letter_or_mark(DS_AT(j, l))) j += l;
+            return j;
+        }
+    }
+    // 3.  ?[\p{P}\p{S}]+[\r\n]*
+    {
+        uint32_t j = i;
+        bool ok = ds_punct_or_symbol(c);
+        if (!ok && cp0 == ' ' && ds_punct_or_symbol(DS_AT(i + 1, l))) { j = i + 1; ok = true; }
+        if (ok) {
+            while (ds_punct_or_symbol(DS_AT(j, l))) j += l;
+            while (DS_AT(j, l) == DS_WS && (s[j] == '\n' || s[j] == '\r')) ++j;
+            return j;
+        }
+    }
+    // 4-6. whitespace run starting at i
+    if (c == DS_WS) {
+        uint32_t j = i, last_nl_end = 0, last_start = i, count = 0;
+        while (DS_AT(j, l) == DS_WS) {
+            last_start = j;
+            const bool nl = s[j] == '\n' || s[j] == '\r';
+            j += l;
+            ++count;
+            if (nl) last_nl_end = j;
+        }
+        if (last_nl_end) return last_nl_end;   // 4. \s*[\r\n]+
+        if (DS_AT(j, l) == kDsEnd) return j;      // 5. \s+(?!\S): the run reaches the end of the stage piece
+        if (count >= 2) return last_start;     // 5. give back one char so that whitespace follows
+        return j;                              // 6. \s+
+    }
+    // no alternative matches at i (an "other" character not followed by a letter or mark): the gap runs up to the next character
+    // where one does
+    uint32_t j = i + len0;
+    for (uint32_t lj; DS_AT(j, lj) == DS_OTHER && !ds_letter_or_mark(DS_AT(j + lj, l)); j += lj) {}
+    return j;
+#undef SMGX_AT_END
+#undef DS_AT
+}
+// Anchor rule (DESIGN §4c): a piece certainly starts at the first character of every digit run and every kana/CJK run, at the first
+// character after either, and at every character that is not a letter or mark after one that is.  pc / c: classes with the kana flag.
+SMGX_HD bool deepseek_anchor_rule(uint8_t pc, uint8_t c) {
+    return (c == DS_N) != (pc == DS_N) || (c & DS_KANA) != (pc & DS_KANA) || (ds_letter_or_mark(pc & 7) && !ds_letter_or_mark(c & 7));
+}
+// Is byte i of the request s[beg..) an anchor?  Same contract as is_anchor_r50k.
+SMGX_HD bool is_anchor_deepseek(const uint8_t* s, uint32_t i, uint32_t beg, const uint8_t* flags, const UnicodeView& u) {
+    if (i == beg) return true;
+    if (flags != nullptr && flags[i - 1] >= 2) return true;
+    uint32_t l;
+    const uint8_t c = ds_class(utf8_decode(s, i, i + 4, l), u);
+    const uint8_t pc = ds_class(prev_cp(s, i, beg), u);
+    return deepseek_anchor_rule(pc, c);
 }
 
 // ---- vocabulary tables ---------------------------------------------------------------------------------------

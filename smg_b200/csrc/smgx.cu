@@ -1634,8 +1634,9 @@ static std::vector<std::pair<std::string, uint32_t>> collect_specials(const char
 }
 // smgx_pretokenizer → Pretok; an unknown value is an invalid argument
 static Pretok pretok_of(smgx_pretokenizer pt) {
-    SMGX_REQUIRE(pt == SMGX_PRETOK_CL100K || pt == SMGX_PRETOK_R50K || pt == SMGX_PRETOK_QWEN2, "Invalid arguments: unknown pretokenizer " + std::to_string((int)pt));
-    return pt == SMGX_PRETOK_R50K ? Pretok::R50k : pt == SMGX_PRETOK_QWEN2 ? Pretok::Qwen2 : Pretok::Cl100k;
+    SMGX_REQUIRE(pt == SMGX_PRETOK_CL100K || pt == SMGX_PRETOK_R50K || pt == SMGX_PRETOK_QWEN2 || pt == SMGX_PRETOK_DEEPSEEK,
+                 "Invalid arguments: unknown pretokenizer " + std::to_string((int)pt));
+    return pt == SMGX_PRETOK_R50K ? Pretok::R50k : pt == SMGX_PRETOK_QWEN2 ? Pretok::Qwen2 : pt == SMGX_PRETOK_DEEPSEEK ? Pretok::DeepSeek : Pretok::Cl100k;
 }
 smgx_status smgx_tokenizer_load_tiktoken_file_ex(smgx_policy* p, const char* model_key, const char* path, const char* const* special_strs,
                                                  const uint32_t* special_ids, uint32_t n_special, smgx_pretokenizer pretokenizer, char** err) {

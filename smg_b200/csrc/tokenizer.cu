@@ -7,6 +7,7 @@
 #include <sstream>
 #include <unordered_map>
 
+#include "deepseek_tables.h"
 #include "nfc_tables.h"
 #include "unicode_tables.h"
 
@@ -235,6 +236,114 @@ __device__ __forceinline__ uint32_t next_piece_window_r50k(const uint8_t* __rest
 #undef WIN_END
 }
 
+// Window form of next_piece_deepseek, same contract as next_piece_window.  s_cls holds ds_class() (kana flag included) | length << 4.
+__device__ __forceinline__ uint32_t next_piece_window_deepseek(const uint8_t* __restrict__ s_txt, const uint8_t* __restrict__ s_cls,
+                                                               const uint8_t* __restrict__ s_stop, uint32_t k, uint32_t W, bool ends_text) {
+#define WIN_NEED(j) do { if ((j) >= W && !ends_text) return kBail; } while (0)
+#define WIN_END(j) ((j) >= W || s_stop[(j)])
+#define WIN_AT(j) (WIN_END(j) ? kDsEnd : ds_stage_class(s_cls[(j)] & 0x0F, z))
+    const uint8_t c0 = s_cls[k] & 0x0F;
+    const uint32_t len0 = s_cls[k] >> 4;
+    const uint8_t b0 = s_txt[k];
+    // Split 1: \p{N}{1,3}
+    if (c0 == DS_N) {
+        uint32_t j = k + len0;
+        for (int c = 1; c < 3; ++c) {
+            WIN_NEED(j);
+            if (WIN_END(j) || (s_cls[j] & 0x0F) != DS_N) break;
+            j += s_cls[j] >> 4;
+        }
+        return j;
+    }
+    // Split 3 inside the stage piece of zone z
+    const uint8_t z = c0 & DS_KANA, c = c0 & 7;
+    // 1. [ASCII punctuation][A-Za-z]+
+    if (b0 < 0x80 && ds_punct_or_symbol(c)) {
+        uint32_t j = k + 1;
+        for (;;) {
+            WIN_NEED(j);
+            if (WIN_END(j) || !is_ascii_letter(s_txt[j])) break;
+            ++j;
+        }
+        if (j > k + 1) return j;
+    }
+    // 2. [^\r\n\p{L}\p{P}\p{S}]?[\p{L}\p{M}]+
+    {
+        uint32_t j = k;
+        bool ok = ds_letter_or_mark(c);
+        if (!ok && !ds_punct_or_symbol(c) && b0 != '\n' && b0 != '\r') {
+            WIN_NEED(k + len0);
+            if (ds_letter_or_mark(WIN_AT(k + len0))) { j = k + len0; ok = true; }
+        }
+        if (ok) {
+            for (;;) {
+                WIN_NEED(j);
+                if (!ds_letter_or_mark(WIN_AT(j))) break;
+                j += s_cls[j] >> 4;
+            }
+            return j;
+        }
+    }
+    // 3.  ?[\p{P}\p{S}]+[\r\n]*
+    {
+        uint32_t j = k;
+        bool ok = ds_punct_or_symbol(c);
+        if (!ok && b0 == ' ') {
+            WIN_NEED(k + 1);
+            if (ds_punct_or_symbol(WIN_AT(k + 1))) { j = k + 1; ok = true; }
+        }
+        if (ok) {
+            for (;;) {
+                WIN_NEED(j);
+                if (!ds_punct_or_symbol(WIN_AT(j))) break;
+                j += s_cls[j] >> 4;
+            }
+            for (;;) {
+                WIN_NEED(j);
+                if (WIN_AT(j) != DS_WS || !(s_txt[j] == '\n' || s_txt[j] == '\r')) break;
+                ++j;
+            }
+            return j;
+        }
+    }
+    // 4-6. whitespace run starting at k
+    if (c == DS_WS) {
+        uint32_t j = k, last_nl_end = 0;
+        for (;;) {
+            WIN_NEED(j);
+            if (WIN_AT(j) != DS_WS) break;
+            const bool nl = s_txt[j] == '\n' || s_txt[j] == '\r';
+            j += s_cls[j] >> 4;
+            if (nl) last_nl_end = j;
+        }
+        if (last_nl_end) return last_nl_end;   // 4. \s*[\r\n]+
+        if (WIN_AT(j) == kDsEnd) return j;     // 5. \s+(?!\S): the run reaches the end of the stage piece
+        if (j == k + len0) return j;           // 6. \s+: a single whitespace character
+        do --j; while (s_cls[j] == kCont);     // 5. give back the last character so that whitespace follows
+        return j;
+    }
+    // a gap: "other" characters up to the first where an alternative matches
+    uint32_t j = k + len0;
+    for (;;) {
+        WIN_NEED(j);
+        if (WIN_AT(j) != DS_OTHER) break;
+        const uint32_t j1 = j + (s_cls[j] >> 4);
+        WIN_NEED(j1);
+        if (ds_letter_or_mark(WIN_AT(j1))) break;
+        j = j1;
+    }
+    return j;
+#undef WIN_NEED
+#undef WIN_END
+#undef WIN_AT
+}
+
+// The global-memory DeepSeek matcher runs only for pieces that cross a window; as a call rather than inlined into the replay loop it keeps
+// the kernel from spilling (inlined, ptxas holds the kernel at 32 registers and spills the replay loop's state).
+__device__ __noinline__ uint32_t next_piece_deepseek_global(const uint8_t* s, uint32_t i, uint32_t n, UnicodeView u, const uint8_t* stop) {
+    return next_piece_deepseek(s, i, n, u, stop);
+}
+
 // One kernel per pattern: the instantiations share the window classification, anchor packing and piece flush, and differ in the anchor
 // rule and the two matchers.
 template <Pretok P>
@@ -259,6 +368,9 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
         s_flag[threadIdx.x] = fl;
         s_stop[threadIdx.x] = fl == 2;
         if ((b & 0xC0) == 0x80) s_cls[threadIdx.x] = kCont;
+        else if constexpr (P == Pretok::DeepSeek) {   // v.uni holds the deepseek_tables.h ranges
+            uint32_t l; const uint32_t cp = utf8_decode(text, i, rend, l); s_cls[threadIdx.x] = (uint8_t)(ds_class(cp, v.uni) | (l << 4));
+        }
         else { uint32_t l; const uint32_t cp = utf8_decode(text, i, rend, l); s_cls[threadIdx.x] = (uint8_t)(char_class(cp, v.uni) | (l << 4)); }
     }
     __syncthreads();
@@ -272,9 +384,11 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
         int q = (int)k - 1;
         while (q >= 0 && s_cls[q] == kCont) --q;
         if (q >= 0) pc = s_cls[q] & 0x0F;
+        else if constexpr (P == Pretok::DeepSeek) pc = ds_class(prev_cp(text, gi, beg), v.uni);
         else pc = char_class(prev_cp(text, gi, beg), v.uni);
         if constexpr (P == Pretok::R50k) return r50k_anchor_rule(pc, k ? s_txt[k - 1] : text[gi - 1], c, s_txt[k]);
         else if constexpr (P == Pretok::Qwen2) return qwen2_anchor_rule(pc, c);
+        else if constexpr (P == Pretok::DeepSeek) return deepseek_anchor_rule(pc, c);
         else return (pc == CH_LETTER && c != CH_LETTER) || (c == CH_NUMBER) != (pc == CH_NUMBER);
     };
     // phase 1: which bytes are anchors?  They are then packed densely, so that phase 2 — the serial regex replay — runs with full
@@ -301,12 +415,14 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
                     uint32_t e;
                     if constexpr (P == Pretok::R50k) e = next_piece_window_r50k(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
                     else if constexpr (P == Pretok::Qwen2) e = next_piece_window<1>(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
+                    else if constexpr (P == Pretok::DeepSeek) e = next_piece_window_deepseek(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
                     else e = next_piece_window<3>(s_txt, s_cls, s_stop, p - cstart, W, ends_text);
                     if (e != kBail) q = cstart + e;
                 }
                 if (q == kBail) {   // the piece looks beyond the window
                     if constexpr (P == Pretok::R50k) q = next_piece_r50k(text, p, rend, v.uni, flags);
                     else if constexpr (P == Pretok::Qwen2) q = next_piece_qwen2(text, p, rend, v.uni, flags);
+                    else if constexpr (P == Pretok::DeepSeek) q = next_piece_deepseek_global(text, p, rend, v.uni, flags);
                     else q = next_piece_cl100k(text, p, rend, v.uni, flags);
                 }
                 const uint32_t slot = atomicAdd(&s_count, 1u);
@@ -317,6 +433,7 @@ __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8
                 else if (q - cstart < W) stop = s_flag[q - cstart] == 2 || anchor_at(q - cstart);
                 else if constexpr (P == Pretok::R50k) stop = flags[q] == 2 || is_anchor_r50k(text, q, beg, flags, v.uni);
                 else if constexpr (P == Pretok::Qwen2) stop = flags[q] == 2 || is_anchor_qwen2(text, q, beg, flags, v.uni);
+                else if constexpr (P == Pretok::DeepSeek) stop = flags[q] == 2 || is_anchor_deepseek(text, q, beg, flags, v.uni);
                 else stop = flags[q] == 2 || is_anchor(text, q, beg, flags, v.uni);
                 if (stop) live = false; else p = q;
             }
@@ -1029,9 +1146,11 @@ void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<
     up(d_pieces_, pieces.data(), pieces.size() * sizeof(PieceSlot));
     up(d_blob_, blob.data(), blob.size());
     up(d_specials_, sp.data(), sp.size() * sizeof(SpecialTok));
-    up(d_uni_lo_, kUniLo, sizeof(kUniLo));
-    up(d_uni_hi_, kUniHi, sizeof(kUniHi));
-    up(d_uni_cls_, kUniCls, sizeof(kUniCls));
+    // the class table of the pre-tokenizer: DeepSeek's chain uses the classes of `tokenizers` (ds_class), the other patterns char_class
+    const bool ds = pretok_ == Pretok::DeepSeek;
+    up(d_uni_lo_, ds ? kDsLo : kUniLo, ds ? sizeof(kDsLo) : sizeof(kUniLo));
+    up(d_uni_hi_, ds ? kDsHi : kUniHi, ds ? sizeof(kDsHi) : sizeof(kUniHi));
+    up(d_uni_cls_, ds ? kDsCls : kUniCls, ds ? sizeof(kDsCls) : sizeof(kUniCls));
     dview_.byte_token = d_byte_token_.as<uint32_t>();
     dview_.pairs = d_pairs_.as<PairSlot>();
     dview_.pair_mask = qmask;
@@ -1042,7 +1161,7 @@ void Tokenizer::build(const std::vector<std::string>& tokens, const std::vector<
     dview_.specials = d_specials_.as<SpecialTok>();
     dview_.n_special = (uint32_t)sp.size();
     for (int i = 0; i < 8; ++i) dview_.special_first[i] = first_bits[i];
-    dview_.uni = UnicodeView{d_uni_lo_.as<uint32_t>(), d_uni_hi_.as<uint32_t>(), d_uni_cls_.as<uint8_t>(), kUniRanges};
+    dview_.uni = UnicodeView{d_uni_lo_.as<uint32_t>(), d_uni_hi_.as<uint32_t>(), d_uni_cls_.as<uint8_t>(), ds ? kDsRanges : kUniRanges};
     if (nfc_) {   // the NFC tables, one allocation (every array 16-byte aligned)
         std::vector<uint8_t> t;
         auto put = [&t](const void* src, size_t bytes) {
@@ -1195,6 +1314,8 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
                 pretokenize_kernel<Pretok::R50k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             else if (pretok_ == Pretok::Qwen2)
                 pretokenize_kernel<Pretok::Qwen2><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+            else if (pretok_ == Pretok::DeepSeek)
+                pretokenize_kernel<Pretok::DeepSeek><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             else
                 pretokenize_kernel<Pretok::Cl100k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());

@@ -453,6 +453,13 @@ LLAMA3_SPLIT_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|
 # Qwen2 / Qwen2.5 / Qwen3 / QwQ: the Llama-3 pattern with \p{N} in place of \p{N}{1,3} (every digit is a piece of its own)
 QWEN2_SPLIT_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|\s+(?!\S)|\s+")
 _SPLIT_PATTERNS = {LLAMA3_SPLIT_PATTERN: _lib.PRETOK_CL100K, QWEN2_SPLIT_PATTERN: _lib.PRETOK_QWEN2}
+# DeepSeek V2 / V2.5 / Coder-V2 / V3 / V3.1 / R1: three Isolated Splits chained — digit triples, kana/CJK runs (U+4E00-U+9FA5,
+# U+3040-U+30FF), then words with punctuation — as the JSON strings of their tokenizer.json decode (the CR and LF are literal characters).
+DEEPSEEK_SPLIT_PATTERNS = (
+    "\\p{N}{1,3}",
+    "[一-龥぀-ゟ゠-ヿ]+",
+    "[!\"#$%&'()*+,\\-./:;<=>?@\\[\\\\\\]^_`{|}~][A-Za-z]+|[^\r\n\\p{L}\\p{P}\\p{S}]?[\\p{L}\\p{M}]+| ?[\\p{P}\\p{S}]+[\r\n]*|\\s*[\r\n]+|"
+    "\\s+(?!\\S)|\\s+")
 
 
 def _byte_level_decoder():
@@ -486,6 +493,46 @@ def _hf_pretokenizer(pre):
         raise ValueError("tokenizer.json: pre_tokenizer must be Split(Llama-3 or Qwen2 regex, Isolated) + ByteLevel(use_regex=False), "
                          "or ByteLevel(use_regex=True, add_prefix_space=False) alone")
     return _SPLIT_PATTERNS[split[0]["pattern"]["Regex"]]
+
+
+def _hf_deepseek_pretokenizer(pre):
+    """True for DeepSeek's pre_tokenizer, Sequence[Split(DEEPSEEK_SPLIT_PATTERNS[0]), Split([1]), Split([2]), ByteLevel], every Split
+    Isolated and not inverted, ByteLevel with use_regex = false and add_prefix_space = false (trim_offsets either way); False when the
+    pre_tokenizer has fewer than two Splits; ValueError naming the difference for any other chain of Splits."""
+    steps = pre.get("pretokenizers", []) if pre.get("type") == "Sequence" else [pre]
+    kinds = [s.get("type") for s in steps]
+    if kinds.count("Split") < 2:
+        return False
+    want = "Sequence[Split(\\p{N}{1,3}), Split(kana/CJK), Split(DeepSeek word regex), ByteLevel]"
+    if kinds != ["Split", "Split", "Split", "ByteLevel"]:
+        raise ValueError(f"tokenizer.json: a chain of Splits is supported only as DeepSeek's {want}, not {kinds}")
+    for k, (s, pat) in enumerate(zip(steps, DEEPSEEK_SPLIT_PATTERNS)):
+        if s.get("pattern") != {"Regex": pat}:
+            raise ValueError(f"tokenizer.json: Split {k} of the chain has pattern {s.get('pattern')!r}; DeepSeek's {want} needs {pat!r}")
+        if str(s.get("behavior")).lower() != "isolated" or s.get("invert"):
+            raise ValueError(f"tokenizer.json: Split {k} of the chain must be Isolated with invert = false, not behavior "
+                             f"{s.get('behavior')!r}, invert {s.get('invert')!r}")
+    bl = steps[3]
+    if bl.get("use_regex") is not False or bl.get("add_prefix_space") is not False:
+        raise ValueError("tokenizer.json: the ByteLevel step of the DeepSeek chain must have use_regex = false and add_prefix_space = false")
+    return True
+
+
+def _overlapping_added_tokens(a, b):
+    """A string of `a` and one of `b` that can overlap in a text (one inside the other, or a suffix of one that starts the other), or
+    None.  `tokenizers` cuts added tokens marked normalized = false first and the others in what is left, so two such strings make the
+    result depend on the marks even without a normalizer."""
+    prefixes = lambda xs: {s[:k] for s in xs for k in range(1, len(s))}   # noqa: E731
+    substrings = lambda xs: {s[i:k] for s in xs for i in range(len(s)) for k in range(i + 1, len(s) + 1)}   # noqa: E731
+    for xs, ys in ((a, b), (b, a)):
+        pre_ys, sub_ys = prefixes(ys), substrings(ys)
+        for x in xs:
+            if x in sub_ys:
+                return x, next(y for y in ys if x in y)
+            for k in range(1, len(x)):
+                if x[k:] in pre_ys:
+                    return x, next(y for y in ys if y.startswith(x[k:]))
+    return None
 
 
 def _hf_normalizer(norm):
@@ -542,6 +589,8 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
     - byte-level BPE: tokenizer.json with no normalizer or NFC, either Split(Llama-3 / cl100k or Qwen2 regex, Isolated) +
       ByteLevel(use_regex=False) or GPT-2's ByteLevel(use_regex=True, add_prefix_space=False) alone, model BPE without dropout / unk /
       byte_fallback;
+    - DeepSeek V2 / V3 / R1 byte-level BPE: normalizer null or the identity Sequence[], pre_tokenizer the chain of three Splits
+      (_hf_deepseek_pretokenizer) + ByteLevel(use_regex=False); added tokens may mix `normalized` marks when no two of them can overlap;
     - SentencePiece-style BPE (Llama 2, CodeLlama, Mistral, Mixtral, TinyLlama): the legacy normalizer Sequence[Prepend("▁"),
       Replace(" " → "▁")] without a pre_tokenizer, or Metaspace(replacement "▁") without a normalizer (_hf_sentencepiece); model BPE with
       byte_fallback = true, the 256 <0xXX> tokens and "▁" in the vocabulary, ignore_merges = false, no dropout / continuing_subword_prefix /
@@ -561,8 +610,14 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         if mdl.get("type") != "BPE" or mdl.get("dropout") or mdl.get("unk_token") or mdl.get("byte_fallback") or \
                 mdl.get("continuing_subword_prefix") or mdl.get("end_of_word_suffix"):
             raise ValueError("tokenizer.json: only plain byte-level BPE models are supported on the GPU path")
-        norm = _hf_normalizer(j.get("normalizer"))
-        pretok = _hf_pretokenizer(j.get("pre_tokenizer") or {})
+        deepseek = _hf_deepseek_pretokenizer(j.get("pre_tokenizer") or {})
+        if deepseek:   # DeepSeek files carry the identity normalizer, an empty Sequence; it is accepted with this pre_tokenizer only
+            if j.get("normalizer") not in (None, {"type": "Sequence", "normalizers": []}):
+                raise ValueError("tokenizer.json: the DeepSeek pre_tokenizer is supported with normalizer null or an empty Sequence only")
+            norm, pretok = _lib.NORMALIZER_NONE, _lib.PRETOK_DEEPSEEK
+        else:
+            norm = _hf_normalizer(j.get("normalizer"))
+            pretok = _hf_pretokenizer(j.get("pre_tokenizer") or {})
         # NFC goes with the Qwen2 Split or GPT-2's ByteLevel; a Llama-3 Split with a normalizer stays refused, as before
         if norm != _lib.NORMALIZER_NONE and pretok == _lib.PRETOK_CL100K:
             raise ValueError("tokenizer.json: a normalizer is supported with the Qwen2 Split or GPT-2's ByteLevel pre_tokenizer, not the Llama-3 Split")
@@ -577,23 +632,32 @@ class HuggingFaceTokenizer(TiktokenTokenizer):
         offs = np.zeros(len(toks) + 1, dtype=np.uint32)
         np.cumsum([len(t) for t in toks], out=offs[1:])
         blob = np.frombuffer(b"".join(toks), dtype=np.uint8).copy()
-        strs, sp_ids, n_added = self._added_tokens(j, norm != _lib.NORMALIZER_NONE)
+        strs, sp_ids, n_added = self._added_tokens(j, norm != _lib.NORMALIZER_NONE, mixed_ok=deepseek)
         self.growth = 3 if norm != _lib.NORMALIZER_NONE else 1   # NFC can grow text threefold
         mg = _u32(merges)
         self.h.call("smgx_tokenizer_load_bpe_merges_norm", self.model, _p(blob), _p(offs), _p(ids), len(toks), _p(mg), len(merges) // 2,
                     1 if mdl.get("ignore_merges") else 0, strs, _p(sp_ids), n_added, pretok, norm)
 
     @staticmethod
-    def _added_tokens(j, normalizer: bool):
-        """added_tokens → (C strings, ids, count) for the loaders, or ValueError for the kinds the GPU path does not implement."""
+    def _added_tokens(j, normalizer: bool, mixed_ok: bool = False):
+        """added_tokens → (C strings, ids, count) for the loaders, or ValueError for the kinds the GPU path does not implement.
+        mixed_ok (DeepSeek's shape only): accept mixed `normalized` marks as long as no string of one mark can overlap one of the other."""
         added = [(a["content"], a["id"]) for a in j.get("added_tokens", [])]
         for a in j.get("added_tokens", []):
             if a.get("lstrip") or a.get("rstrip") or a.get("single_word"):
                 raise ValueError("tokenizer.json: added tokens with lstrip / rstrip / single_word are not supported")
         # Without a normalizer, `tokenizers` extracts added tokens in one pass over the raw text whether they are marked normalized or
         # not, as long as all of them carry the same mark; a mix splits the text in two passes, which the GPU path does not implement.
-        if len({bool(a.get("normalized", False)) for a in j.get("added_tokens", [])}) > 1:
+        # The two passes give what one pass gives when no string of one mark overlaps a string of the other.
+        marks = {bool(a.get("normalized", False)) for a in j.get("added_tokens", [])}
+        if len(marks) > 1 and not mixed_ok:
             raise ValueError("tokenizer.json: added tokens with mixed `normalized` values are not supported")
+        if len(marks) > 1:
+            clash = _overlapping_added_tokens([a["content"] for a in j["added_tokens"] if a.get("normalized")],
+                                              [a["content"] for a in j["added_tokens"] if not a.get("normalized")])
+            if clash:
+                raise ValueError(f"tokenizer.json: added tokens {clash[0]!r} and {clash[1]!r} have different `normalized` values and can "
+                                 "overlap in a text; `tokenizers` then matches them in two passes, which the GPU path does not implement")
         # With a normalizer, added tokens marked normalized are matched on the normalized text — a second pass the GPU path does not
         # implement.  Those marked normalized = false are cut from the raw text first, which is what the GPU path does.
         if normalizer and any(a.get("normalized", False) for a in j.get("added_tokens", [])):

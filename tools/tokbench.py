@@ -1,10 +1,11 @@
 """bench.py's text-in leg on its own, with the default sizes of bench.py:
-    python tools/tokbench.py [cl100k_base|r50k_base|qwen2|qwen2-nonorm|llama2] [--nfd]
+    python tools/tokbench.py [cl100k_base|r50k_base|qwen2|qwen2-nonorm|llama2|deepseek] [--nfd]
 cl100k_base / r50k_base pick the pre-tokenizer regex over the synthetic tiktoken vocabulary.  qwen2 loads the Qwen2-style tokenizer.json
 fixture (NFC normalizer, single-digit Split); qwen2-nonorm the same file with its normalizer removed, so that the difference is the cost
 of the NFC stage.  llama2 loads the Llama-2-style fixture (▁ normalization, byte fallback; a 1 210-entry vocabulary, not a real 32 000-entry
-one) and also times `tokenizers` encode_batch on the host threads over the corpus's first `batch` documents.  --nfd converts the corpus to
-NFD first, so that every accented letter takes the normalizer's slow path.
+one) and deepseek the DeepSeek-V3-style fixture (the chain of three Splits; an 816-entry vocabulary, not DeepSeek's 128 000 entries); both
+also time `tokenizers` encode_batch on the host threads over the corpus's first `batch` documents.  --nfd converts the corpus to NFD first,
+so that every accented letter takes the normalizer's slow path.
 Prints one JSON line."""
 import functools, sys, os, json, tempfile, unicodedata
 sys.path.insert(0, os.getcwd())
@@ -12,8 +13,9 @@ import bench
 from smg_b200 import CacheAwarePolicy
 enc = sys.argv[1] if len(sys.argv) > 1 and not sys.argv[1].startswith("--") else "cl100k_base"
 nfd = "--nfd" in sys.argv
-if enc.startswith("qwen2") or enc == "llama2":
-    fixture = os.path.join(os.getcwd(), "tests", "golden", "hf_llama2_style_tokenizer.json" if enc == "llama2" else "hf_qwen2_style_tokenizer.json")
+FIXTURES = {"llama2": "hf_llama2_style_tokenizer.json", "deepseek": "hf_deepseek_v3_style_tokenizer.json"}
+if enc.startswith("qwen2") or enc in FIXTURES:
+    fixture = os.path.join(os.getcwd(), "tests", "golden", FIXTURES.get(enc, "hf_qwen2_style_tokenizer.json"))
     if enc == "qwen2-nonorm":
         j = json.load(open(fixture))
         j["normalizer"] = None
@@ -34,7 +36,7 @@ class A: pass
 a=A(); a.batch=4096; a.workers=64; a.text_docs=8192; a.text_bytes=2048; a.steps=2000
 res = bench.text_in_leg(a, 0)
 res.pop("cpu_tokenize_baseline", None)   # always measured with the cl100k regex there
-if enc == "llama2":
+if enc in FIXTURES:
     import time, tokenizers
     ref, texts = tokenizers.Tokenizer.from_file(fixture), corpus[:a.batch]
     ref.encode_batch(texts[:256], add_special_tokens=False)
