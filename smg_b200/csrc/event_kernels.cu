@@ -20,7 +20,7 @@
 //   shared device code     slot probes, worker-set algebra, scan_drain / jump_search (generic search), hash_block
 //   hash_blocks_kernel     the hash stream
 //   event_search_thread_kernel, event_search_warp_kernel
-//   finish_pick, drain_resolve   argmax + store of one request; the register drain of a failed count test (search2 and the lane kernel)
+//   finish_pick, drain_resolve   argmax + store of one request; the register drain of a failed count test (search2 and the warp kernel)
 //   search2_body / event_search2_kernel
 //   alternatives           (SMGX_EVENT_PATH, every one parity-green; on H100 event_lane_kernel below is the default, the pair is `split`)
 //       event_hs_kernel        hash stream whose last CTA per 256-request group searches
@@ -1595,9 +1595,11 @@ __global__ void __launch_bounds__(128, MINB) event_tile_kernel(const __grid_cons
 //      both hashes, both probes in flight together, the count-only jump test (event_tree.rs:720).  A block's content hash depends on
 //      that block alone, so a full hit or a novel request reads 128 B of tokens.  A failed count test goes onto a shared-memory queue
 //      together with what both probes found;
-//   B  the queue is striped over the CTA's 8 warps, two drains per round so that the loads and lookups of the second overlap those of
-//      the first: lane p (1 ≤ p < last) reads and hashes block p and looks it up in the tag array (tag_sector / tag_finish: a slot is
-//      read only where the tag matches), lanes 0 and last take the queued probes, and drain_resolve replays the ordered scan.
+//   B  each warp serves four queued drains at a time, 8 lanes each, in segments of 8 positions: a lane reads and hashes one block and
+//      looks it up in the tag array (tag_sector / tag_finish: a slot is read only where the tag matches), the queued probe of `last`
+//      stands in for its block, and the ordered scan is replayed over the segment.  A drain stops at the segment where the scan stops
+//      (a missing position, an empty active set), so a partial hit reads the blocks up to its stored prefix's end and not the rest;
+//      its slot then takes the next queued drain.
 // What needs the rolling prefix hashes or more than one jump (Multi entries, > 32 blocks, jump_size < blocks − 1) is pushed onto a device
 // queue, at most once per request (from A or from B), and finished by event_slow_kernel right behind.  That kernel is launched only when
 // such a request is possible: the index holds a Multi entry, or the launch allows more than 32 blocks or more than one jump (MultiArgs.skip_slow).
@@ -1623,14 +1625,14 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
     __shared__ int32_t s_slice[64];
     __shared__ uint64_t s_load[64], s_ts[64];
     __shared__ LaneDrain s_q[256];
-    __shared__ uint32_t s_n;
+    __shared__ uint32_t s_n, s_head;   // queued drains; the next drain a free slot of phase B takes
     if (threadIdx.x < 64) {
         bool ok = threadIdx.x < v.n_workers;
         s_slice[threadIdx.x] = ok ? f.slice_of_id[threadIdx.x] : -1;
         s_load[threadIdx.x] = ok ? f.load_of_id[threadIdx.x] : 0;
         s_ts[threadIdx.x] = ok ? v.tree_sizes[threadIdx.x] : 0;
     }
-    if (threadIdx.x == 0) s_n = 0;
+    if (threadIdx.x == 0) { s_n = 0; s_head = 32; }
     __syncthreads();
     const int32_t min_load_idx = f.derived->min_load_idx;
     const uint64_t elig = f.elig[0];
@@ -1669,50 +1671,80 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
     }
     __syncthreads();
 
-    // ---- phase B: one warp per queued drain, the queue striped over the 8 warps, two drains per round ----
-    const int lane = threadIdx.x & 31;
+    // ---- phase B: segments of 8 positions, four drains per warp round ----
+    // Lanes 8d..8d+7 serve drain slot d; in a round, lane 8d+j reads, hashes and looks up position 1 + 8·seg + j of its slot's drain
+    // (seg: the drain's next segment), the position `last` being phase A's probe carried in the queue.  The ordered scan is then replayed
+    // over the segment from the scan state the slot's lanes carry (the active set, the latest drained set and its score).  A drain ends
+    // where the scan ends: at a missing position (nothing after it can change the pick, event_tree.rs:598-604), when the active set is
+    // empty, at an entry that needs the generic search, or once `last` is replayed; its slot then takes the next queued drain.
+    const int lane = threadIdx.x & 31, sub = lane & 7, lead = lane & 24;
+    const unsigned slot_bits = 0xffu << lead;
     const uint32_t n_d = s_n;
-    auto drain_done = [&](const LaneDrain& d, const DrainResult& r) {   // lane 0
-        if (r.bail) { to_slow(d.g); return; }
-        const SimpleLoc l = simple_locate(a, d.g);
-        finish_pick(a.b[l.j], l.r, s_slice, s_load, s_ts, min_load_idx, r.win, r.score, d.ntok);
-    };
-    for (uint32_t q = threadIdx.x >> 5; q < n_d; q += 16) {
-        const bool two = q + 8 < n_d;
-        const LaneDrain& d0 = s_q[q];
-        const LaneDrain& d1 = s_q[two ? q + 8 : q];
-        const int last0 = (int)(d0.ntok >> 4) - 1, last1 = two ? (int)(d1.ntok >> 4) - 1 : -1;   // last1 = -1: no second drain this round
-        const bool m0 = lane >= 1 && lane < last0, m1 = lane >= 1 && lane < last1;
-        // the second block is prefetched into L2 and loaded once the first is hashed: both blocks in registers at once leave too few
-        // for the lookups below (spills at 64 registers)
-        const uint32_t* p1 = m1 ? a.b[simple_locate(a, d1.g).j].tokens + d1.off + (size_t)lane * 16 : nullptr;
-        if (m1) asm volatile("prefetch.global.L2 [%0];\n\tprefetch.global.L2 [%1];" ::"l"(p1), "l"(p1 + 8));
-        uint32_t w0[16], w1[16];
-        uint64_t h0 = 0, h1 = 0;
-        if (m0) { load_block16(a.b[simple_locate(a, d0.g).j].tokens + d0.off + (size_t)lane * 16, w0); h0 = xxh3_16words(w0, kSeed); }
-        if (m1) { load_block16(p1, w1); h1 = xxh3_16words(w1, kSeed); }
-        // positions 1..last-1 of both requests looked up at once in the tags (both tag loads, then both slot loads in flight); about
-        // half of them are absent keys, which then read no slot.  Positions 0 and last are phase A's probes, carried in the queue.
-        const uint32_t rep0 = tag_rep((uint32_t)lane, h0), rep1 = tag_rep((uint32_t)lane, h1);
-        TagCursor c0{0, 0, true}, c1{0, 0, true};
-        if (m0) c0 = tag_sector(v, rep0, slot_hash((uint32_t)lane, h0) & v.mask);
-        if (m1) c1 = tag_sector(v, rep1, slot_hash((uint32_t)lane, h1) & v.mask);
-        Slot sl0{0, 0, SLOT_EMPTY, 0, 0}, sl1{0, 0, SLOT_EMPTY, 0, 0};
-        if (c0.cand) sl0 = load_slot(v.slots + tag_slot(c0));
-        if (c1.cand) sl1 = load_slot(v.slots + tag_slot(c1));
-        bool f0 = false, f1 = false;
-        if (m0) f0 = tag_finish(v, (uint32_t)lane, h0, rep0, c0, sl0, sl0);
-        if (m1) f1 = tag_finish(v, (uint32_t)lane, h1, rep1, c1, sl1, sl1);
-        __syncwarp();   // keeps the queued probes' shared-memory loads here: hoisted above the token loads they cost the registers of a spill
-        if (lane == 0) { f0 = true; sl0.state = SLOT_SINGLE; sl0.payload = d0.p0; f1 = true; sl1.state = SLOT_SINGLE; sl1.payload = d1.p0; }
-        if (lane == last0) { f0 = d0.f1 != 0; sl0.state = SLOT_SINGLE; sl0.payload = d0.p1; }
-        if (lane == last1) { f1 = d1.f1 != 0; sl1.state = SLOT_SINGLE; sl1.payload = d1.p1; }
-        const DrainResult r0 = drain_resolve(last0 + 1, elig, lane, f0, sl0);
-        if (lane == 0) drain_done(d0, r0);
-        if (two) {
-            const DrainResult r1 = drain_resolve(last1 + 1, elig, lane, f1, sl1);
-            if (lane == 0) drain_done(d1, r1);
+    uint32_t qi = (threadIdx.x >> 5) + 8u * (uint32_t)(lane >> 3);   // the first 32 drains spread over the warps; then s_head
+    uint64_t active = qi < n_d ? s_q[qi].p0 : 0, last_set = 0;
+    uint32_t last_score = 0, seg = 0;
+    while (__any_sync(FULL, qi < n_d)) {
+        const bool live = qi < n_d;
+        const LaneDrain& d = s_q[live ? qi : 0];
+        const uint32_t last = live ? (d.ntok >> 4) - 1 : 0, pos = 1 + 8 * seg + (uint32_t)sub;
+        const bool in_range = live && pos <= last;
+        bool found = false;
+        Slot sl{0, 0, SLOT_EMPTY, 0, 0};
+        if (in_range && pos < last) {
+            uint32_t w[16];
+            load_block16(a.b[simple_locate(a, d.g).j].tokens + d.off + (size_t)pos * 16, w);
+            const uint64_t h = xxh3_16words(w, kSeed);
+            const uint32_t rep = tag_rep(pos, h);
+            const TagCursor c = tag_sector(v, rep, slot_hash(pos, h) & v.mask);
+            if (c.cand) sl = load_slot(v.slots + tag_slot(c));
+            found = tag_finish(v, pos, h, rep, c, sl, sl);
         }
+        __syncwarp();   // keeps the queued probe's shared-memory loads here, below the token load
+        if (in_range && pos == last) { found = d.f1 != 0; sl.state = SLOT_SINGLE; sl.payload = d.p1; }
+        // drain_resolve's ballot loop, each slot on its own 8-bit field of the ballots
+        const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
+        unsigned remaining = __ballot_sync(FULL, in_range) & slot_bits;
+        bool bail = false;
+        for (;;) {
+            const uint32_t nact = (uint32_t)__popcll(active);
+            const bool noop = found && sl.state == SLOT_SINGLE && cnt >= nact;   // retain guard (:611, :641)
+            const unsigned bm = __ballot_sync(FULL, in_range && !noop) & remaining;
+            if (!__any_sync(FULL, bm != 0)) break;
+            const int k = bm ? __ffs((int)bm) - 1 : lane;
+            const bool fk = __shfl_sync(FULL, (int)found, k) != 0;
+            const uint32_t sk = __shfl_sync(FULL, sl.state, k);
+            const uint64_t ws = shfl64(sl.payload, k);
+            if (bm) {
+                const uint32_t pk = 1 + 8 * seg + (uint32_t)(k & 7);
+                if (!fk) {                                                         // missing entry drains everything (:598-604)
+                    const uint64_t e = active & elig;
+                    if (e) { last_set = e; last_score = pk; }
+                    active = 0;
+                } else if (sk != SLOT_SINGLE) bail = true;
+                else if ((uint32_t)__popcll(ws) < nact) {
+                    const uint64_t e = active & ~ws & elig;
+                    if (e) { last_set = e; last_score = pk; }
+                    active &= ws;
+                }
+                remaining = (bail || !active) ? 0u : remaining & ~((2u << k) - 1u);
+            }
+        }
+        const bool done = live && (bail || !active || 8 * seg + 8 >= last);
+        if (done && sub == 0) {
+            if (bail) to_slow(d.g);
+            else {
+                uint64_t win = active & elig;
+                uint32_t score = last + 1;
+                if (!win) { win = last_set; score = last_score; }
+                const SimpleLoc l = simple_locate(a, d.g);
+                finish_pick(a.b[l.j], l.r, s_slice, s_load, s_ts, min_load_idx, win, score, d.ntok);
+            }
+            qi = atomicAdd(&s_head, 1u);
+        }
+        qi = __shfl_sync(FULL, qi, lead);
+        if (done) {
+            active = qi < n_d ? s_q[qi].p0 : 0; last_set = 0; last_score = 0; seg = 0;
+        } else ++seg;
     }
 }
 

@@ -10,8 +10,9 @@ one JSON line per K: per kernel name the launches, total and mean time, decision
 kernel-second, then the span of the call on the GPU, the time any kernel ran and the idle time between them.
 
 Bytes model (what the default kernel requests per decision, not DRAM traffic: the probes mostly hit L2): 8 B of offsets, 4 B of pick,
-64 B of tokens for each block hashed (blocks 0 and last for a full hit or a novel request; all of them when the count test fails and
-the drain hashes the rest) and 32 B per slot probe (2 for a full hit or a novel request, 2 + the request's blocks for a drain).
+64 B of tokens for each block hashed and 32 B per slot probe.  A full hit or a novel request hashes and probes blocks 0 and last.  A
+failed count test drains positions 1..last-1 in segments of 8 and stops at the segment holding the first missing position (a partial
+hit keeps k whole blocks, so position k): it hashes and looks up blocks 0, last and every position of the segments it reads.
 Profile in a run of its own: tracing slows the host, so these times are not the bench's.
 """
 import argparse
@@ -27,12 +28,14 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
 
-def bytes_per_decision(kinds, T, bs):
-    """Mean modelled bytes per decision over the ring (kinds: 0 full hit, 1 partial → failed count test, 2 novel)."""
-    P = T // bs
-    tokens = np.where(kinds == 1, 4 * T, 2 * 4 * bs)
-    probes = np.where(kinds == 1, 2 + P, 2)
-    return float((8 + 4 + tokens + 32 * probes).mean())
+def bytes_per_decision(kinds, keeps, T, bs):
+    """Mean modelled bytes per decision over the ring (kinds: 0 full hit, 1 partial → failed count test, 2 novel; keeps: tokens a
+    partial hit keeps)."""
+    last = T // bs - 1
+    stop = np.clip(keeps // bs, 1, last)                                   # the drain's first missing position
+    drained = np.minimum(8 * ((stop - 1) // 8 + 1), last - 1)             # whole segments of 8 up to it, within 1..last-1
+    blocks = np.where(kinds == 1, 2 + drained, 2)
+    return float((8 + 4 + blocks * (4 * bs + 32)).mean())
 
 
 def union_us(spans):
@@ -80,16 +83,16 @@ def main():
     offsets = (np.arange(B + 1, dtype=np.uint64) * T).astype(np.uint32)
     d_off = L.smgx_device_alloc(h.p, offsets.nbytes, C.byref(err))
     h.call("smgx_memcpy_h2d", d_off, offsets.ctypes.data_as(C.c_void_p), offsets.nbytes)
-    d_tok, d_out, kinds_all = [], [], []
+    d_tok, d_out, kinds_all, keeps_all = [], [], [], []
     for r in range(R):
-        q, kinds, _keeps = bench.gen_batch(seqs, B, 42 + r, bs)
-        kinds_all.append(kinds)
+        q, kinds, keeps = bench.gen_batch(seqs, B, 42 + r, bs)
+        kinds_all.append(kinds); keeps_all.append(keeps)
         flat = np.ascontiguousarray(q.reshape(-1))
         dt = L.smgx_device_alloc(h.p, flat.nbytes, C.byref(err))
         h.call("smgx_memcpy_h2d", dt, flat.ctypes.data_as(C.c_void_p), flat.nbytes)
         d_tok.append(dt)
         d_out.append(L.smgx_device_alloc(h.p, B * 4, C.byref(err)))
-    model_bytes = bytes_per_decision(np.concatenate(kinds_all), T, bs)
+    model_bytes = bytes_per_decision(np.concatenate(kinds_all), np.concatenate(keeps_all), T, bs)
 
     for K in [int(k) for k in args.steps.split(",")]:
         order = [i % R for i in range(K)]
