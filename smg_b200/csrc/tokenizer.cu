@@ -17,16 +17,28 @@ namespace {
 
 constexpr uint32_t kInvalidTok = 0xFFFFFFFFu;
 
+// Per-request kernels (the K1a candidates, pre-tokenizer, NFC and ▁ stages) run on a grid of request_grid(chunks, n): blockIdx.x = 256-byte
+// chunk of the request, one thread per byte; the request index is folded over y and z because gridDim.y is capped at 65535, and
+// request_index() unfolds it.  The last z slice can hold up to gridDim.z - 1 indices ≥ n: those CTAs return before reading offsets.
+constexpr uint32_t kMaxGridY = 65535;
+dim3 request_grid(uint32_t chunks, uint32_t n) {
+    SMGX_REQUIRE(n >= 1 && (uint64_t)n <= (uint64_t)kMaxGridY * kMaxGridY, "request grid: batch size out of range");   // gridDim.z ≤ 65535 too
+    const uint32_t z = (uint32_t)(((uint64_t)n + kMaxGridY - 1) / kMaxGridY);
+    return dim3(chunks, (n + z - 1) / z, z);
+}
+__device__ __forceinline__ uint32_t request_index() { return blockIdx.z * gridDim.y + blockIdx.y; }
+
 // ---- K1a: pre-tokenisation, parallel over bytes ---------------------------------------------------------------
-// Grid: blockIdx.y = request, blockIdx.x = 256-byte chunk of that request, one thread per byte.
 // Special tokens first (tiktoken `encode`: the regex only ever sees the text between two specials):
 //   special_candidates_kernel   does a special string start at this byte?  (longest at a position)
 //   special_resolve_kernel      one warp per request: accept candidates left to right, dropping those inside an accepted span
 //   flags: 0 ordinary byte, 1 piece start, 2 first byte of a special, 3 inside a special, 4 unresolved candidate
 __global__ void __launch_bounds__(256) special_candidates_kernel(BpeView v, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                                 uint8_t* __restrict__ flags, uint32_t* __restrict__ tmp_ids,
+                                                                 uint32_t n, uint8_t* __restrict__ flags, uint32_t* __restrict__ tmp_ids,
                                                                  uint64_t* __restrict__ tmp_rk) {
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t i = beg + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rend) return;
     const uint8_t c = text[i];
@@ -348,14 +360,17 @@ __device__ __noinline__ uint32_t next_piece_deepseek_global(const uint8_t* s, ui
 // rule and the two matchers.
 template <Pretok P>
 __global__ void __launch_bounds__(256) pretokenize_kernel(BpeView v, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                          uint8_t* __restrict__ flags, Piece* __restrict__ pieces, uint32_t* __restrict__ n_pieces) {
+                                                          uint32_t n, uint8_t* __restrict__ flags, Piece* __restrict__ pieces,
+                                                          uint32_t* __restrict__ n_pieces) {
     __shared__ Piece s_list[320];
     __shared__ uint32_t s_anchor[256];
     __shared__ uint32_t s_wcnt[8];
     __shared__ uint32_t s_count, s_base;
     __shared__ uint8_t s_txt[256], s_cls[256], s_stop[256], s_flag[256];
+    const uint32_t r = request_index();
+    if (r >= n) return;
     if (threadIdx.x == 0) s_count = 0;
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     const uint32_t i = cstart + threadIdx.x;
     const uint32_t W = cstart < rend ? min(256u, rend - cstart) : 0;
@@ -736,8 +751,10 @@ constexpr uint32_t kNfcShort = 32;
 struct NfcLong { uint32_t start, end, req; };
 
 __global__ void __launch_bounds__(256) nfc_check_kernel(NfcView nv, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                        const uint8_t* __restrict__ flags, uint32_t* __restrict__ dirty) {
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+                                                        uint32_t n, const uint8_t* __restrict__ flags, uint32_t* __restrict__ dirty) {
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t i = beg + blockIdx.x * blockDim.x + threadIdx.x;
     if (beg + blockIdx.x * blockDim.x >= rend) return;   // CTA-uniform
     bool bad = false;
@@ -760,11 +777,14 @@ __device__ __forceinline__ uint32_t block_sum_256(uint32_t x, uint32_t* s_w) {
 }
 
 __global__ void __launch_bounds__(256) nfc_segment_kernel(NfcView nv, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                          uint32_t first_byte, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ dirty,
-                                                          uint32_t* __restrict__ seg_len, uint32_t* __restrict__ chunk_sum, uint32_t* __restrict__ nlen,
-                                                          uint8_t* __restrict__ norm_tmp, NfcLong* __restrict__ longs, uint32_t* __restrict__ n_long) {
+                                                          uint32_t n, uint32_t first_byte, const uint8_t* __restrict__ flags,
+                                                          const uint32_t* __restrict__ dirty, uint32_t* __restrict__ seg_len,
+                                                          uint32_t* __restrict__ chunk_sum, uint32_t* __restrict__ nlen, uint8_t* __restrict__ norm_tmp,
+                                                          NfcLong* __restrict__ longs, uint32_t* __restrict__ n_long) {
     __shared__ uint32_t s_w[8];
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     if (cstart >= rend) return;
     if (!dirty[r]) {
@@ -831,14 +851,16 @@ __global__ void __launch_bounds__(256) nfc_long_kernel(NfcView nv, const uint8_t
     }
 }
 
-__global__ void __launch_bounds__(256) nfc_write_kernel(const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets, uint32_t first_byte,
-                                                        const uint8_t* __restrict__ flags, const uint32_t* __restrict__ tmp_ids,
+__global__ void __launch_bounds__(256) nfc_write_kernel(const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets, uint32_t n,
+                                                        uint32_t first_byte, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ tmp_ids,
                                                         const uint32_t* __restrict__ dirty, const uint32_t* __restrict__ seg_len,
                                                         const uint32_t* __restrict__ chunk_sum, const uint8_t* __restrict__ norm_tmp,
                                                         const uint32_t* __restrict__ noff, uint8_t* __restrict__ ntext, uint8_t* __restrict__ nflags,
                                                         uint32_t* __restrict__ nids) {
     __shared__ uint32_t s_w[8];
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     if (cstart >= rend) return;
     const uint32_t i = cstart + threadIdx.x;
@@ -888,10 +910,12 @@ __global__ void __launch_bounds__(256) nfc_write_kernel(const uint8_t* __restric
 //                        single symbol is already its token, longer pieces go to the merge kernels' lists by symbol count
 // and bpe_merge_kernel<true> / bpe_long_kernel<true> merge them.
 __global__ void __launch_bounds__(256) ms_count_kernel(MetaspaceMode mm, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                       uint32_t first_byte, const uint8_t* __restrict__ flags, uint32_t* __restrict__ chunk_sum,
-                                                       uint32_t* __restrict__ nlen) {
+                                                       uint32_t n, uint32_t first_byte, const uint8_t* __restrict__ flags,
+                                                       uint32_t* __restrict__ chunk_sum, uint32_t* __restrict__ nlen) {
     __shared__ uint32_t s_w[8];
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     if (cstart >= rend) return;   // CTA-uniform
     const uint32_t i = cstart + threadIdx.x;
@@ -903,11 +927,14 @@ __global__ void __launch_bounds__(256) ms_count_kernel(MetaspaceMode mm, const u
 }
 
 __global__ void __launch_bounds__(256) ms_write_kernel(MetaspaceMode mm, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                       uint32_t first_byte, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ tmp_ids,
-                                                       const uint32_t* __restrict__ chunk_sum, const uint32_t* __restrict__ noff,
-                                                       uint8_t* __restrict__ ntext, uint8_t* __restrict__ nflags, uint32_t* __restrict__ nids) {
+                                                       uint32_t n, uint32_t first_byte, const uint8_t* __restrict__ flags,
+                                                       const uint32_t* __restrict__ tmp_ids, const uint32_t* __restrict__ chunk_sum,
+                                                       const uint32_t* __restrict__ noff, uint8_t* __restrict__ ntext, uint8_t* __restrict__ nflags,
+                                                       uint32_t* __restrict__ nids) {
     __shared__ uint32_t s_w[8];
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     if (cstart >= rend) return;
     const uint32_t i = cstart + threadIdx.x;
@@ -933,8 +960,10 @@ __global__ void __launch_bounds__(256) ms_write_kernel(MetaspaceMode mm, const u
 }
 
 __global__ void __launch_bounds__(256) ms_symbolize_kernel(BpeView v, uint32_t split, const uint8_t* __restrict__ text, const uint32_t* __restrict__ offsets,
-                                                           uint8_t* __restrict__ flags, uint32_t* __restrict__ tmp_ids) {
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+                                                           uint32_t n, uint8_t* __restrict__ flags, uint32_t* __restrict__ tmp_ids) {
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t i = beg + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rend || flags[i] >= 2 || (text[i] & 0xC0) == 0x80) return;
     uint32_t ns;
@@ -942,10 +971,12 @@ __global__ void __launch_bounds__(256) ms_symbolize_kernel(BpeView v, uint32_t s
     if (ms_piece_start(text, flags, i, beg, split)) flags[i] = 1;   // neighbours only test flags >= 2: 0 → 1 does not change their answer
 }
 
-__global__ void __launch_bounds__(256) ms_emit_kernel(const uint32_t* __restrict__ offsets, const uint8_t* __restrict__ flags,
+__global__ void __launch_bounds__(256) ms_emit_kernel(const uint32_t* __restrict__ offsets, uint32_t n, const uint8_t* __restrict__ flags,
                                                       const uint32_t* __restrict__ tmp_ids, Piece* __restrict__ pieces, uint32_t* __restrict__ counters,
                                                       uint32_t* __restrict__ totals, uint32_t* __restrict__ miss_short, uint32_t* __restrict__ miss_long) {
-    const uint32_t r = blockIdx.y, beg = offsets[r], rend = offsets[r + 1];
+    const uint32_t r = request_index();
+    if (r >= n) return;
+    const uint32_t beg = offsets[r], rend = offsets[r + 1];
     const uint32_t cstart = beg + blockIdx.x * blockDim.x;
     if (cstart >= rend) return;   // CTA-uniform: the warps below stay whole
     const uint32_t i = cstart + threadIdx.x;
@@ -1210,9 +1241,9 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
         SMGX_CUDA(cudaMemsetAsync(sc.flags.ptr, 0, total_bytes, stream));
     }
     {
-        const dim3 grid2((max_len + 255) / 256, n);
+        const dim3 grid2 = request_grid((max_len + 255) / 256, n);
         if (dview_.n_special && max_len) {
-            special_candidates_kernel<<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, sc.flags.as<uint8_t>(), sc.tmp_ids.as<uint32_t>(),
+            special_candidates_kernel<<<grid2, 256, 0, stream>>>(dview_, d_text, d_offsets, n, sc.flags.as<uint8_t>(), sc.tmp_ids.as<uint32_t>(),
                                                                sc.tmp_rk.as<uint64_t>());
             SMGX_CUDA(cudaGetLastError());
             ++*launches;
@@ -1252,12 +1283,13 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
             uint32_t* chunk_sum = (uint32_t*)(b + o_chunk);
             uint8_t* norm_tmp = b + o_tmp;
             NfcLong* longs = (NfcLong*)(b + o_long);
-            nfc_check_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, flags, dirty);
-            nfc_segment_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, first_byte, flags, dirty, seg_len, chunk_sum, nlen, norm_tmp, longs, n_long);
+            nfc_check_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, n, flags, dirty);
+            nfc_segment_kernel<<<grid2, 256, 0, stream>>>(nview_, d_text, d_offsets, n, first_byte, flags, dirty, seg_len, chunk_sum, nlen, norm_tmp, longs,
+                                                          n_long);
             const unsigned sms = current_sm_count();
             nfc_long_kernel<<<sms, 256, 0, stream>>>(nview_, d_text, d_offsets, first_byte, longs, n_long, (uint32_t*)(b + o_ent), seg_len, chunk_sum, nlen, norm_tmp);
             scan_counts_kernel<<<1, 1024, 0, stream>>>(nlen, n, noff);
-            nfc_write_kernel<<<grid2, 256, 0, stream>>>(d_text, d_offsets, first_byte, flags, tmp_ids, dirty, seg_len, chunk_sum, norm_tmp, noff,
+            nfc_write_kernel<<<grid2, 256, 0, stream>>>(d_text, d_offsets, n, first_byte, flags, tmp_ids, dirty, seg_len, chunk_sum, norm_tmp, noff,
                                                         b + o_text, b + o_flags, (uint32_t*)(b + o_ids));
             SMGX_CUDA(cudaGetLastError());
             *launches += 5;
@@ -1280,9 +1312,9 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
             uint32_t* noff = nlen + n;
             uint32_t* chunk_sum = (uint32_t*)(b + o_chunk);   // indexed from first_byte
             SMGX_CUDA(cudaMemsetAsync(nlen, 0, (size_t)n * 4, stream));
-            ms_count_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, first_byte, flags, chunk_sum, nlen);
+            ms_count_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, n, first_byte, flags, chunk_sum, nlen);
             scan_counts_kernel<<<1, 1024, 0, stream>>>(nlen, n, noff);
-            ms_write_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, first_byte, flags, tmp_ids, chunk_sum, noff, b + o_text, b + o_flags,
+            ms_write_kernel<<<grid2, 256, 0, stream>>>(ms_, d_text, d_offsets, n, first_byte, flags, tmp_ids, chunk_sum, noff, b + o_text, b + o_flags,
                                                        (uint32_t*)(b + o_ids));
             SMGX_CUDA(cudaGetLastError());
             *launches += 3;
@@ -1295,29 +1327,30 @@ void Tokenizer::encode_batch(const uint8_t* d_text, const uint32_t* d_offsets, u
         SMGX_CUDA(cudaMemsetAsync(sc.n_pieces.ptr, 0, 16, stream));
         if (max_len && ms_.on) {
             // segmenter + symbolizer instead of the pre-tokenizer and the whole-piece lookup, then the merge tiers by symbol count
-            const dim3 gridn((len_bound + 255) / 256, n);   // CTAs past a request's normalized end return at once
+            const dim3 gridn = request_grid((len_bound + 255) / 256, n);   // CTAs past a request's normalized end return at once
             const unsigned sms = current_sm_count();
             const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)span / 2 + 255) / 256 + 1, sms * 16ull);
             uint32_t* cnt = sc.n_pieces.as<uint32_t>();
             uint32_t* miss_short = sc.miss.as<uint32_t>();
             uint32_t* miss_long = miss_short + span + 1;
-            ms_symbolize_kernel<<<gridn, 256, 0, stream>>>(dview_, ms_.split, text, offsets, flags, tmp_ids);
-            ms_emit_kernel<<<gridn, 256, 0, stream>>>(offsets, flags, tmp_ids, sc.pieces.as<Piece>(), cnt, sc.totals.as<uint32_t>(), miss_short, miss_long);
+            ms_symbolize_kernel<<<gridn, 256, 0, stream>>>(dview_, ms_.split, text, offsets, n, flags, tmp_ids);
+            ms_emit_kernel<<<gridn, 256, 0, stream>>>(offsets, n, flags, tmp_ids, sc.pieces.as<Piece>(), cnt, sc.totals.as<uint32_t>(), miss_short, miss_long);
             bpe_merge_kernel<true><<<std::min(grid, sms * 4), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_short, tmp_ids, sc.totals.as<uint32_t>());
             bpe_long_kernel<true><<<std::min(grid, sms * 8), 256, 0, stream>>>(dview_, text, sc.pieces.as<Piece>(), cnt, miss_long, tmp_ids,
                                                                           sc.tmp_rk.as<uint64_t>(), sc.totals.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             *launches += 4;
         } else if (max_len) {
-            const dim3 gridp((len_bound + 255) / 256, n);   // with NFC: CTAs past a request's normalized end find an empty window
+            const dim3 gridp = request_grid((len_bound + 255) / 256, n);   // with NFC: CTAs past a request's normalized end find an empty window
             if (pretok_ == Pretok::R50k)
-                pretokenize_kernel<Pretok::R50k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::R50k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, n, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             else if (pretok_ == Pretok::Qwen2)
-                pretokenize_kernel<Pretok::Qwen2><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::Qwen2><<<gridp, 256, 0, stream>>>(dview_, text, offsets, n, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             else if (pretok_ == Pretok::DeepSeek)
-                pretokenize_kernel<Pretok::DeepSeek><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::DeepSeek><<<gridp, 256, 0, stream>>>(dview_, text, offsets, n, flags, sc.pieces.as<Piece>(),
+                                                                                sc.n_pieces.as<uint32_t>());
             else
-                pretokenize_kernel<Pretok::Cl100k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
+                pretokenize_kernel<Pretok::Cl100k><<<gridp, 256, 0, stream>>>(dview_, text, offsets, n, flags, sc.pieces.as<Piece>(), sc.n_pieces.as<uint32_t>());
             SMGX_CUDA(cudaGetLastError());
             ++*launches;
             // the piece count lives on the device, so the grids are sized for the worst case the text allows and stride over the lists
