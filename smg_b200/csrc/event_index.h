@@ -4,10 +4,22 @@
 // keeps `DashMap<(position, ContentHash), SeqEntry>` whose values own FxHashSet<u32> worker sets; here the index
 // is ONE open-addressed table of 32-byte slots in HBM (one sector per probe) with worker sets as bitsets:
 //
-//   Slot   { u64 content_hash; u32 position; u32 state; u64 prefix_hash; u64 payload }         32 B, 32 B-aligned
+//   Slot   { u64 content_hash; u32 position; u32 state; u32 run; u32 pad; u64 payload }          32 B, 32 B-aligned
 //          state SINGLE: SeqEntry::Single(prefix_hash, set)   payload = the bitset itself when the fleet has ≤ 64
 //                                                              interned workers, else a row number into `rows`
 //          state MULTI : SeqEntry::Multi(map)                  payload = head of a linked list in `multi`
+//          run: the entry's record in `runs` (kNil for none).  A Single entry's prefix_hash is host-only (`prefix_`, parallel
+//          to the slots): no kernel reads it
+//   runs   [n_runs] RunRec { u64 content_hash; u32 position; u32 state; u64 payload; u64 pad }  32 B, append-only
+//          each apply_stored call reserves one run of consecutive records, one per block in position order, so that within a
+//          run record index = anchor + position.  A block that creates its key fills its record and the slot's `run` points at
+//          it; a block whose key already exists leaves its record dead (state EMPTY).  A live record (SINGLE / MULTI) exists only
+//          for a key that is live in the slots, with the slot's state and payload: keys are unique, so a key match in ANY live
+//          record is that entry, wherever the record lies.  A drain reads the records of a stored sequence's positions as one
+//          contiguous range from the anchor of its position-0 slot, in the same round trip as their tokens, where the slots
+//          are one cold HBM read each behind a tag round trip.  Compacted whole runs at a time (runs with no live record are
+//          dropped, records never move inside a run) at a rebuild, or when dead records outnumber live entries and the arena has
+//          doubled since the last compaction
 //   rows   [n_rows][words] u64                                 worker bitsets (words = ceil(workers/64) → pow2, ≤ 32)
 //   multi  { u64 prefix_hash; u64 payload; u32 next; ... }     32 B nodes; one per distinct prefix hash
 //   tree_sizes[worker] u64                                     event_tree.rs:264
@@ -41,8 +53,16 @@ struct alignas(32) Slot {
     uint64_t content;
     uint32_t pos;
     uint32_t state;
-    uint64_t prefix;
+    uint32_t run;
+    uint32_t pad;
     uint64_t payload;
+};
+struct alignas(32) RunRec {
+    uint64_t content;
+    uint32_t pos;
+    uint32_t state;   // the slot's state while the key is live in it; SLOT_EMPTY for a dead record
+    uint64_t payload;
+    uint64_t pad;
 };
 struct alignas(32) MultiNode {
     uint64_t prefix;
@@ -51,7 +71,7 @@ struct alignas(32) MultiNode {
     uint32_t pad0;
     uint64_t pad1;
 };
-static_assert(sizeof(Slot) == 32 && sizeof(MultiNode) == 32, "32-byte records");
+static_assert(sizeof(Slot) == 32 && sizeof(MultiNode) == 32 && sizeof(RunRec) == 32, "32-byte records");
 
 // What the kernels see.
 struct EventIndexView {
@@ -60,6 +80,8 @@ struct EventIndexView {
     const MultiNode* multi;
     const uint64_t* tree_sizes;
     const uint8_t* tags; // one tag per slot (see above)
+    const RunRec* runs;  // the run arena (see above)
+    uint32_t n_runs;     // records in it
     uint32_t mask;       // capacity - 1
     uint32_t words;      // u64 words per worker bitset
     uint32_t n_workers;  // interned workers
@@ -109,7 +131,9 @@ public:
     // Push pending writes to the device in `stream` order and return the view for kernels.
     EventIndexView flush(cudaStream_t stream, uint64_t* launches);
     bool device_enabled = true;
-    bool pending() const { return full_dirty_ || tree_dirty_ || !dirty_slots_.empty() || !dirty_multi_.empty() || !dirty_rows_.empty(); }
+    bool pending() const {
+        return full_dirty_ || tree_dirty_ || !dirty_slots_.empty() || !dirty_multi_.empty() || !dirty_rows_.empty() || !dirty_runs_.empty();
+    }
 
 private:
     // bitset helpers on the HOST mirror
@@ -121,17 +145,30 @@ private:
 
     int64_t find_slot(uint32_t pos, uint64_t content) const;
     uint32_t insert_slot(uint32_t pos, uint64_t content);
-    void insert_entry(uint32_t pos, uint64_t content, uint64_t prefix, uint32_t wid);
+    void insert_entry(uint32_t pos, uint64_t content, uint64_t prefix, uint32_t wid, uint32_t i);
     void drop_entry(const BlockRec& r, uint32_t wid);
     uint32_t new_multi(uint64_t prefix, uint64_t payload, uint32_t next);
     void rebuild(uint32_t new_capacity, uint32_t new_words);
-    void mark_slot(uint32_t i) { if (!full_dirty_) dirty_slots_.push_back(i); }
+    void compact_runs();
+    // every write to a slot's state or payload goes through here: it rewrites the slot's record as well
+    void mark_slot(uint32_t i) {
+        if (!full_dirty_) dirty_slots_.push_back(i);
+        const Slot& s = slots_[i];
+        if (s.run == kNil) return;
+        const bool live = s.state == SLOT_SINGLE || s.state == SLOT_MULTI;
+        runs_[s.run] = RunRec{s.content, s.pos, live ? s.state : (uint32_t)SLOT_EMPTY, live ? s.payload : 0, 0};
+        if (!full_dirty_) dirty_runs_.push_back(s.run);
+    }
     void mark_multi(uint32_t i) { if (!full_dirty_) dirty_multi_.push_back(i); }
     void mark_row(uint32_t i) { if (!full_dirty_) dirty_rows_.push_back(i); }
 
     uint32_t jump_;
     uint32_t words_ = 1;
     std::vector<Slot> slots_;
+    std::vector<uint64_t> prefix_;        // a Single entry's prefix hash, per slot (host only)
+    std::vector<RunRec> runs_;
+    std::vector<uint32_t> run_starts_;    // first record of each run, ascending
+    size_t runs_kept_ = 0;                // records left by the last compaction
     uint32_t mask_ = 0;
     uint64_t live_ = 0, tombs_ = 0, multi_slots_ = 0;
     std::vector<uint64_t> rows_;
@@ -144,14 +181,14 @@ private:
     uint64_t workers_version_ = 0;
 
     // device mirror
-    DevBuf d_slots_, d_rows_, d_multi_, d_tree_, d_tags_;
+    DevBuf d_slots_, d_rows_, d_multi_, d_tree_, d_tags_, d_runs_;
     PinBuf stage_;
     DevBuf d_stage_;
     cudaEvent_t stage_done_ = nullptr;
     bool stage_pending_ = false;
     bool full_dirty_ = true;
     bool tree_dirty_ = true;
-    std::vector<uint32_t> dirty_slots_, dirty_multi_, dirty_rows_;
+    std::vector<uint32_t> dirty_slots_, dirty_multi_, dirty_rows_, dirty_runs_;
 };
 
 }  // namespace smgx

@@ -62,7 +62,7 @@ __device__ __forceinline__ Slot load_slot(const Slot* p) {
     uint4 a = __ldg(q), b = __ldg(q + 1);
     Slot s;
     s.content = mk64(a.x, a.y); s.pos = a.z; s.state = a.w;
-    s.prefix = mk64(b.x, b.y); s.payload = mk64(b.z, b.w);
+    s.run = b.x; s.pad = b.y; s.payload = mk64(b.z, b.w);
     return s;
 }
 __device__ __forceinline__ MultiNode load_node(const MultiNode* p) {
@@ -1611,7 +1611,8 @@ __device__ __forceinline__ SimpleLoc simple_locate(const MultiArgs& a, uint32_t 
     return l;
 }
 
-struct LaneDrain { uint32_t g, off, ntok, f1; uint64_t p0, p1; };   // a failed count test: request, token range, the probes of blocks 0 and last
+// a failed count test: request, token range, the probes of blocks 0 and last, the run-arena anchor of block 0's entry
+struct LaneDrain { uint32_t g, off, ntok, f1; uint64_t p0, p1; uint32_t anchor; };
 
 // queues request g for event_slow_kernel; a launch that skipped that kernel (a.skip_slow) reports it as an internal error instead (a bit
 // OR-ed into err_flag, as the over-the-cap 1 of these kernels is, so that neither clears the other)
@@ -1665,7 +1666,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
                 if (f1 && s1.state != SLOT_SINGLE) to_slow(g);
                 else if (f1 && __popcll(s1.payload) == __popcll(s0.payload))   // count-only jump test (:720)
                     finish_pick(b, loc.r, s_slice, s_load, s_ts, min_load_idx, s0.payload & elig, nb, ntok);
-                else s_q[atomicAdd(&s_n, 1u)] = LaneDrain{g, off, ntok, (uint32_t)f1, s0.payload, s1.payload};
+                else s_q[atomicAdd(&s_n, 1u)] = LaneDrain{g, off, ntok, (uint32_t)f1, s0.payload, s1.payload, s0.run};
             }
         }
     }
@@ -1682,25 +1683,46 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
     const uint32_t n_d = s_n;
     uint32_t qi = (threadIdx.x >> 5) + 8u * (uint32_t)(lane >> 3);   // the first 32 drains spread over the warps; then s_head
     uint64_t active = qi < n_d ? s_q[qi].p0 : 0, last_set = 0;
-    uint32_t last_score = 0, seg = 0;
+    uint32_t last_score = 0, seg = 0, anchor = qi < n_d ? s_q[qi].anchor : kNil;
     while (__any_sync(FULL, qi < n_d)) {
         const bool live = qi < n_d;
         const LaneDrain& d = s_q[live ? qi : 0];
         const uint32_t last = live ? (d.ntok >> 4) - 1 : 0, pos = 1 + 8 * seg + (uint32_t)sub;
         const bool in_range = live && pos <= last;
         bool found = false;
-        Slot sl{0, 0, SLOT_EMPTY, 0, 0};
+        uint32_t reanchor = kNil;
+        Slot sl{0, 0, SLOT_EMPTY, kNil, 0, 0};
         if (in_range && pos < last) {
+            // the record the run layout puts at this position, loaded beside the tokens (neither depends on the hash): where it
+            // is a live record of the key, it is the entry (event_index.h), and the tag walk and the cold slot are skipped
+            const uint32_t ri = anchor + pos;
+            uint4 ra = make_uint4(0, 0, SLOT_EMPTY, 0);
+            uint2 rb = make_uint2(0, 0);
+            if (ri < v.n_runs) {
+                const uint4* q = reinterpret_cast<const uint4*>(v.runs + ri);
+                ra = __ldg(q);
+                rb = __ldg(reinterpret_cast<const uint2*>(q + 1));
+            }
             uint32_t w[16];
             load_block16(a.b[simple_locate(a, d.g).j].tokens + d.off + (size_t)pos * 16, w);
             const uint64_t h = xxh3_16words(w, kSeed);
-            const uint32_t rep = tag_rep(pos, h);
-            const TagCursor c = tag_sector(v, rep, slot_hash(pos, h) & v.mask);
-            if (c.cand) sl = load_slot(v.slots + tag_slot(c));
-            found = tag_finish(v, pos, h, rep, c, sl, sl);
+            if (mk64(ra.x, ra.y) == h && ra.z == pos && ra.w != SLOT_EMPTY) {
+                found = true; sl.state = ra.w; sl.payload = mk64(rb.x, rb.y);
+            } else {
+                const uint32_t rep = tag_rep(pos, h);
+                const TagCursor c = tag_sector(v, rep, slot_hash(pos, h) & v.mask);
+                if (c.cand) sl = load_slot(v.slots + tag_slot(c));
+                found = tag_finish(v, pos, h, rep, c, sl, sl);
+                if (found && sl.run != kNil) reanchor = sl.run - pos;   // the run that holds this position, for the next segments
+            }
         }
         __syncwarp();   // keeps the queued probe's shared-memory loads here, below the token load
         if (in_range && pos == last) { found = d.f1 != 0; sl.state = SLOT_SINGLE; sl.payload = d.p1; }
+        {   // a slot's lanes that found their key outside the anchored run re-anchor the drain at the highest such position
+            const unsigned rbits = __ballot_sync(FULL, reanchor != kNil) & slot_bits;
+            const uint32_t ra = __shfl_sync(FULL, reanchor, rbits ? 31 - __clz((int)rbits) : lane);
+            if (rbits) anchor = ra;
+        }
         // drain_resolve's ballot loop, each slot on its own 8-bit field of the ballots
         const uint32_t cnt = (found && sl.state == SLOT_SINGLE) ? (uint32_t)__popcll(sl.payload) : 0;
         unsigned remaining = __ballot_sync(FULL, in_range) & slot_bits;
@@ -1743,7 +1765,7 @@ __global__ void __launch_bounds__(256, 4) event_lane_kernel(const __grid_constan
         }
         qi = __shfl_sync(FULL, qi, lead);
         if (done) {
-            active = qi < n_d ? s_q[qi].p0 : 0; last_set = 0; last_score = 0; seg = 0;
+            active = qi < n_d ? s_q[qi].p0 : 0; last_set = 0; last_score = 0; seg = 0; anchor = qi < n_d ? s_q[qi].anchor : kNil;
         } else ++seg;
     }
 }

@@ -10,9 +10,12 @@ one JSON line per K: per kernel name the launches, total and mean time, decision
 kernel-second, then the span of the call on the GPU, the time any kernel ran and the idle time between them.
 
 Bytes model (what the default kernel requests per decision, not DRAM traffic: the probes mostly hit L2): 8 B of offsets, 4 B of pick,
-64 B of tokens for each block hashed and 32 B per slot probe.  A full hit or a novel request hashes and probes blocks 0 and last.  A
-failed count test drains positions 1..last-1 in segments of 8 and stops at the segment holding the first missing position (a partial
-hit keeps k whole blocks, so position k): it hashes and looks up blocks 0, last and every position of the segments it reads.
+64 B of tokens for each block hashed and 32 B per lookup.  A full hit or a novel request hashes blocks 0 and last and probes their
+slots.  A failed count test drains positions 1..last-1 in segments of 8 and stops at the segment holding the first missing position (a
+partial hit keeps k whole blocks, so position k): it hashes blocks 0, last and every position of the segments it reads, and reads the
+32 B run-arena record of each drained position (contiguous records from the anchor of block 0's entry) in place of its slot; a
+position whose record misses (the missing one, or a run broken by another store) adds a 1 B tag and, where the tag matches, a slot,
+which this model does not count.
 Profile in a run of its own: tracing slows the host, so these times are not the bench's.
 """
 import argparse
@@ -34,7 +37,7 @@ def bytes_per_decision(kinds, keeps, T, bs):
     last = T // bs - 1
     stop = np.clip(keeps // bs, 1, last)                                   # the drain's first missing position
     drained = np.minimum(8 * ((stop - 1) // 8 + 1), last - 1)             # whole segments of 8 up to it, within 1..last-1
-    blocks = np.where(kinds == 1, 2 + drained, 2)
+    blocks = np.where(kinds == 1, 2 + drained, 2)                        # each: 64 B of tokens + a 32 B slot (0, last) or record (drained)
     return float((8 + 4 + blocks * (4 * bs + 32)).mean())
 
 
