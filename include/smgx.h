@@ -431,8 +431,29 @@ smgx_status smgx_select_batch_tokens(smgx_policy* p, const char* model_key, cons
  *       fleet instead of all landing on one worker, (score, load) tie-breaks read the running loads and the f32 imbalance gate is
  *       re-evaluated per request.  Batches handed over in one smgx_select_many_tokens_device call form one stream.  The bumps are not
  *       kept: the next call starts from the snapshot of its own smgx_set_fleet_state.  Not available with duplicate URLs in the slice,
- *       for mapped submissions or for sharded candidates. */
+ *       for mapped submissions or for sharded candidates.
+ * smgx_set_load_feedback and smgx_set_load_feedback_policies set ONE state and the last call wins: smgx_set_load_feedback(p, e) is
+ * the mask "event-driven calls only, if e", smgx_set_load_feedback_policies(p, 0) turns every stream off. */
 smgx_status smgx_set_load_feedback(smgx_policy* p, int enabled, char** err);
+/* Load feedback per policy: the gateway names the picks its router follows with a WorkerLoadGuard — the HTTP router guards cache_aware
+ * picks (routers/http/router.rs:319-321), the gRPC router every pick (routers/grpc/context.rs:248-259).
+ *   SMGX_FEEDBACK_CACHE_AWARE: every cache_aware mode — the event-driven calls as smgx_set_load_feedback(p, 1) does, and the token-tree and
+ *       string-tree modes (smgx_select_batch_tokens, smgx_submit_tokens, smgx_select_batch_text, smgx_submit_text,
+ *       smgx_select_batch_request_text, an event-mode model whose indexer is empty).  Request i of a call is decided as select_worker would
+ *       decide it with the snapshot loads plus one per pick of requests < i: the f32 imbalance gate, the min-load picks and the fallback to
+ *       the first healthy worker read the running loads.  Not with SMGX_TREE_BATCH_SNAPSHOT (no interleaving of concurrent select_worker
+ *       calls reads snapshot trees with streamed loads): the setter, and a tree-mode call that meets the combination, return
+ *       SMGX_INVALID_ARGUMENT.
+ *   SMGX_FEEDBACK_PREFIX_HASH: smgx_prefix_hash_select_batch_tokens and smgx_prefix_hash_select_many_tokens_device (every batch of one call
+ *       forms one stream): the bound (Σ load + 1) / n × load_factor, the ring worker's load_ok and the least loaded fallback read the running loads.
+ *   SMGX_FEEDBACK_POWER_OF_TWO: smgx_power_of_two_select_batch: same draws and pairs; the request-count comparison reads the running loads.
+ * The gRPC router sets all three bits, the HTTP router SMGX_FEEDBACK_CACHE_AWARE only.  The prefix_hash and power_of_two passes keep the
+ * running loads in shared memory: a worker slice of more than 25 600 entries is SMGX_INVALID_ARGUMENT with their bit set.
+ * The bumps are not kept after the call.  Any other bit is SMGX_INVALID_ARGUMENT. */
+#define SMGX_FEEDBACK_CACHE_AWARE 1u
+#define SMGX_FEEDBACK_PREFIX_HASH 2u
+#define SMGX_FEEDBACK_POWER_OF_TWO 4u
+smgx_status smgx_set_load_feedback_policies(smgx_policy* p, uint32_t mask, char** err);
 /* Pipelined form for the host batcher: up to smgx_pipeline_depth() submissions may be in flight; each owns a stream
  * and device staging.  Buffers must stay valid (and should be pinned) until smgx_wait(ticket) returns. */
 uint32_t smgx_pipeline_depth(const smgx_policy* p);

@@ -237,6 +237,11 @@ public:
     void add_worker(const Worker& w) { char* err = nullptr; detail::check(smgx_add_worker(h_->p, normalize_model_key(w.model_id()).c_str(), w.url().c_str(), &err), err); }   // :252-266
     void remove_worker_by_url(const std::string& url) { char* err = nullptr; detail::check(smgx_remove_worker(h_->p, "", url.c_str(), &err), err); }                            // :302-308 (no-op)
     void evict_cache(size_t max_size) { char* err = nullptr; detail::check(smgx_evict_cache(h_->p, max_size, &err), err); }                                                      // :311-352
+    // Batches as the request stream of a router that guards every cache_aware pick (WorkerLoadGuard): request i sees the fleet snapshot
+    // plus the picks of requests < i, in every mode (event-driven, token tree, string tree).  Needs SMGX_TREE_BATCH_SEQUENTIAL.
+    void set_load_feedback_all_modes(bool enabled) {
+        char* err = nullptr; detail::check(smgx_set_load_feedback_policies(h_->p, enabled ? SMGX_FEEDBACK_CACHE_AWARE : 0u, &err), err);
+    }
 
     std::shared_ptr<KvEventMonitor> kv_event_monitor() { return std::make_shared<KvEventMonitor>(h_); }
     void set_kv_event_monitor(std::shared_ptr<KvEventMonitor> m) {       // :213-215
@@ -388,6 +393,10 @@ public:
         detail::check(smgx_prefix_hash_configure(h_->p, config.prefix_token_count, config.load_factor, &err), err);
     }
     static PrefixHashPolicy with_defaults() { return PrefixHashPolicy(); }   // :100-103
+    // batches as the request stream of a router that guards every pick (gRPC): the bound and the fallback read the running loads
+    void set_load_feedback(bool enabled) {
+        char* err = nullptr; detail::check(smgx_set_load_feedback_policies(h_->p, enabled ? SMGX_FEEDBACK_PREFIX_HASH : 0u, &err), err);
+    }
     const char* name() const override { return "prefix_hash"; }              // :231-233
     // the registry's per-model ring (SelectWorkerInfo.hash_ring), bound to this policy's device state
     std::shared_ptr<HashRing> hash_ring(const std::vector<std::string>& urls, const std::string& model = UNKNOWN_MODEL_ID) {
@@ -444,6 +453,10 @@ public:
         h_ = std::make_shared<detail::Handle>(c);
     }
     const char* name() const override { return "power_of_two"; }             // :122-124
+    // batches as the request stream of a router that guards every pick (gRPC): the request-count comparison reads the running loads
+    void set_load_feedback(bool enabled) {
+        char* err = nullptr; detail::check(smgx_set_load_feedback_policies(h_->p, enabled ? SMGX_FEEDBACK_POWER_OF_TWO : 0u, &err), err);
+    }
     // update_loads (:129-135): url → WorkerLoadResponse::effective_token_usage() (the mean token_usage over the DP ranks; 0.0 for none)
     void update_loads(const std::map<std::string, double>& token_usage) {
         if (token_usage.empty()) return;

@@ -152,6 +152,7 @@ def load():
     sig("smgx_select_batch_text", st, vp, cp, vp, vp, u32, vp, vp, vp, vp, u32, pp)
     sig("smgx_select_batch_tokens", st, vp, cp, vp, vp, u32, vp, vp, pp)
     sig("smgx_set_load_feedback", st, vp, C.c_int, pp)
+    sig("smgx_set_load_feedback_policies", st, vp, u32, pp)
     sig("smgx_pipeline_depth", u32, vp)
     sig("smgx_submit_tokens", st, vp, cp, vp, vp, u32, vp, vp, P(u64), pp)
     sig("smgx_wait", st, vp, u64, pp)

@@ -42,11 +42,40 @@ __global__ void __launch_bounds__(256) power_of_two_kernel(const P2cArgs a) {
     if (a.out_metric) a.out_metric[i] = metric;
 }
 
+// Load feedback (smgx_set_load_feedback_policies, SMGX_FEEDBACK_POWER_OF_TWO): the gRPC router guards every pick (routers/grpc/context.rs:248-259),
+// so request i compares loads that include the picks of requests < i.  The draws and the pairs do not depend on loads and come from
+// power_of_two_kernel; this pass walks the requests in order with the running loads in shared memory and redoes the request-count
+// comparison (metric 0: (double)load, first candidate on ties); token-usage comparisons and single-worker picks keep their result.  Then the
+// pick's load is bumped.  The comparison chain is serial, so one thread walks it; the warp stages the loads.
+__global__ void __launch_bounds__(32) power_of_two_feedback_kernel(const P2cArgs a, uint32_t n_slice) {
+    extern __shared__ uint64_t s_L[];   // [n_slice]
+    for (uint32_t i = threadIdx.x; i < n_slice; i += 32) s_L[i] = a.loads[i];
+    __syncwarp();
+    if (threadIdx.x != 0) return;
+    for (uint32_t i = 0; i < a.n; ++i) {
+        int32_t out = a.out_idx[i];
+        if (a.out_metric[i] == 0) {
+            const int32_t c1 = a.out_pair[2 * i], c2 = a.out_pair[2 * i + 1];
+            out = (double)s_L[c1] <= (double)s_L[c2] ? c1 : c2;                          // :79-95
+            a.out_idx[i] = out;
+        }
+        if (out >= 0) ++s_L[out];
+    }
+}
+
 }  // namespace
 
 void launch_power_of_two(const P2cArgs& a, cudaStream_t stream) {
     if (!a.n) return;
     power_of_two_kernel<<<(a.n + 255) / 256, 256, 0, stream>>>(a);
+    SMGX_CUDA(cudaGetLastError());
+}
+
+void launch_power_of_two_feedback(const P2cArgs& a, uint32_t n_slice, cudaStream_t stream) {
+    if (!a.n) return;
+    const size_t smem = (size_t)(n_slice ? n_slice : 1) * 8;
+    if (smem > 48 * 1024) SMGX_CUDA(cudaFuncSetAttribute(power_of_two_feedback_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    power_of_two_feedback_kernel<<<1, 32, smem, stream>>>(a, n_slice);
     SMGX_CUDA(cudaGetLastError());
 }
 

@@ -18,5 +18,9 @@ struct P2cArgs {
     uint8_t* out_metric;      // device [n] or nullptr: 0 = request_count, 1 = token_usage, 2 = no comparison made
 };
 void launch_power_of_two(const P2cArgs& a, cudaStream_t stream);
+// load feedback: after launch_power_of_two, redo the request-count comparisons in request order on running loads (out_pair and out_metric
+// must be set); the n_slice loads must fit in shared memory (kMaxP2cFeedbackSlice)
+constexpr uint32_t kMaxP2cFeedbackSlice = 200 * 1024 / 8;
+void launch_power_of_two_feedback(const P2cArgs& a, uint32_t n_slice, cudaStream_t stream);
 
 }  // namespace smgx

@@ -141,6 +141,45 @@ __global__ void __launch_bounds__(kHashThreads) prefix_hash_kernel(const __grid_
     }
 }
 
+// HashRing::find_healthy_url (hash_ring.rs:102-134) of a request's prefix hash over the slice's healthy workers: its ring candidate,
+// -1 when no ring URL resolves to a healthy slice entry.  Shared by the pick kernel and the load-feedback candidate kernel.
+__device__ __forceinline__ int32_t ring_candidate(const RingView& ring, const PrefixFleetView& fleet, uint64_t ph) {
+    int32_t initial = -1;
+    // key = format!("{prefix_hash:016x}"): 16 lower-case hex digits, most significant first, as one blake3 block
+    uint32_t m[16];
+#pragma unroll
+    for (int wd = 0; wd < 4; ++wd) {
+        uint32_t word = 0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const uint32_t nib = (uint32_t)(ph >> (60 - 4 * (4 * wd + c))) & 15u;
+            word |= (nib < 10 ? '0' + nib : 'a' + nib - 10) << (8 * c);
+        }
+        m[wd] = word;
+    }
+#pragma unroll
+    for (int wd = 4; wd < 16; ++wd) m[wd] = 0;
+    uint32_t cv[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) cv[q] = b3::kIV[q];
+    b3::compress(cv, m, 0, 16, b3::CHUNK_START | b3::CHUNK_END | b3::ROOT);
+    const uint64_t key_pos = mk64(cv[0], cv[1]);
+    // partition_point(|pos| pos < key_pos): positions are uniform 64-bit hashes, so a table of "first entry at or above
+    // bucket b's lower bound" (2+ buckets per entry) lands within an entry or two of the answer — two dependent loads, not 14
+    const uint32_t bk = (uint32_t)(key_pos >> ring.bucket_shift);
+    uint32_t lo = __ldg(ring.bucket + bk);
+    const uint32_t hi = __ldg(ring.bucket + bk + 1);
+    while (lo < hi && __ldg(ring.pos + lo) < key_pos) ++lo;
+    uint32_t e = lo == ring.len ? 0 : lo;
+    for (uint32_t step = 0; step < ring.len; ++step) {
+        int32_t s = __ldg(ring.slice + e);
+        while (s >= 0 && !(fleet.flags[s] & 1)) s = fleet.dup_prev[s];   // the URL resolves to its last HEALTHY slice entry
+        if (s >= 0) { initial = s; break; }
+        if (++e == ring.len) e = 0;
+    }
+    return initial;
+}
+
 // K-prefix-2: one thread per request: ring lookup + bounded-load pick from bt.hash[r]
 __global__ void __launch_bounds__(kThreads) prefix_pick_kernel(const RingView ring, const PrefixFleetView fleet, const __grid_constant__ PrefixArgs a) {
     const PrefixBatch& bt = a.b[blockIdx.y];
@@ -156,41 +195,7 @@ __global__ void __launch_bounds__(kThreads) prefix_pick_kernel(const RingView ri
     else if (!some) branch = SMGX_PH_NO_TOKENS;                         // :213-216
     else if (d.n_healthy == 0) branch = SMGX_PH_NO_HEALTHY_WORKERS;     // :143-145
     else {
-        int32_t initial = -1;
-        if (ring.has_ring && ring.len) {
-            // key = format!("{prefix_hash:016x}"): 16 lower-case hex digits, most significant first, as one blake3 block
-            uint32_t m[16];
-#pragma unroll
-            for (int wd = 0; wd < 4; ++wd) {
-                uint32_t word = 0;
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const uint32_t nib = (uint32_t)(ph >> (60 - 4 * (4 * wd + c))) & 15u;
-                    word |= (nib < 10 ? '0' + nib : 'a' + nib - 10) << (8 * c);
-                }
-                m[wd] = word;
-            }
-#pragma unroll
-            for (int wd = 4; wd < 16; ++wd) m[wd] = 0;
-            uint32_t cv[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) cv[q] = b3::kIV[q];
-            b3::compress(cv, m, 0, 16, b3::CHUNK_START | b3::CHUNK_END | b3::ROOT);
-            const uint64_t key_pos = mk64(cv[0], cv[1]);
-            // partition_point(|pos| pos < key_pos): positions are uniform 64-bit hashes, so a table of "first entry at or above
-            // bucket b's lower bound" (2+ buckets per entry) lands within an entry or two of the answer — two dependent loads, not 14
-            const uint32_t bk = (uint32_t)(key_pos >> ring.bucket_shift);
-            uint32_t lo = __ldg(ring.bucket + bk);
-            const uint32_t hi = __ldg(ring.bucket + bk + 1);
-            while (lo < hi && __ldg(ring.pos + lo) < key_pos) ++lo;
-            uint32_t e = lo == ring.len ? 0 : lo;
-            for (uint32_t step = 0; step < ring.len; ++step) {
-                int32_t s = __ldg(ring.slice + e);
-                while (s >= 0 && !(fleet.flags[s] & 1)) s = fleet.dup_prev[s];   // the URL resolves to its last HEALTHY slice entry
-                if (s >= 0) { initial = s; break; }
-                if (++e == ring.len) e = 0;
-            }
-        }
+        const int32_t initial = (ring.has_ring && ring.len) ? ring_candidate(ring, fleet, ph) : -1;
         if (initial >= 0) {
             if (load_ok(fleet.loads[initial], d)) { idx = initial; branch = SMGX_PH_RING_HIT; }
             else { idx = d.least_ok >= 0 ? d.least_ok : initial; branch = SMGX_PH_LOAD_BALANCE_WALK; }
@@ -207,6 +212,100 @@ __global__ void __launch_bounds__(kThreads) prefix_pick_kernel(const RingView ri
 // (load, idx) lexicographic minimum = Iterator::min_by_key's FIRST minimum
 __device__ __forceinline__ void take_min(uint64_t& load, int32_t& idx, uint64_t ol, int32_t oi) {
     if (oi >= 0 && (idx < 0 || ol < load || (ol == load && oi < idx))) { load = ol; idx = oi; }
+}
+
+// ---- load feedback (smgx_set_load_feedback_policies, SMGX_FEEDBACK_PREFIX_HASH): the batch as the request stream of a router that guards
+// every pick (routers/grpc/context.rs:248-259), request i seeing the snapshot loads plus one per pick of requests < i ----
+constexpr int64_t kPhNoRing = -1;     // no ring, or no ring URL resolves to a healthy slice entry → least loaded healthy worker
+constexpr int64_t kPhDecided = -2;    // None (no worker, no tokens, no healthy worker): written by the candidate kernel
+
+// phase 1, one thread per request: everything prefix_pick_kernel decides without loads.  bt.hash[r] is replaced by the request's ring
+// candidate, kPhNoRing or kPhDecided.
+__global__ void __launch_bounds__(kThreads) prefix_candidate_kernel(const RingView ring, const PrefixFleetView fleet, const __grid_constant__ PrefixArgs a) {
+    const PrefixBatch& bt = a.b[blockIdx.y];
+    const uint32_t r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= bt.n || !bt.out_idx) return;
+    const uint64_t ph = bt.hash[r];
+    const uint32_t n_tok = __ldg(bt.offsets + r + 1) - __ldg(bt.offsets + r);
+    const bool some = n_tok != 0 && (bt.has_tokens == nullptr || bt.has_tokens[r] != 0);
+    int64_t cand = kPhDecided;
+    uint8_t branch = SMGX_PH_NO_HEALTHY_WORKERS;
+    if (fleet.n_slice == 0) branch = SMGX_PH_NO_HEALTHY_WORKERS;             // :208-210
+    else if (!some) branch = SMGX_PH_NO_TOKENS;                              // :213-216
+    else if (fleet.derived->n_healthy != 0) cand = (ring.has_ring && ring.len) ? ring_candidate(ring, fleet, ph) : kPhNoRing;   // else :143-145
+    bt.hash[r] = (uint64_t)cand;
+    if (cand != kPhDecided) return;
+    bt.out_idx[r] = -1;
+    if (bt.out_info) {
+        smgx_decision_info o;
+        o.matched = 0; o.input = n_tok; o.branch = branch; o.nodes = 0; o.reserved[0] = o.reserved[1] = 0;
+        bt.out_info[r] = o;
+    }
+}
+
+// phase 2, one warp, the requests of every batch of the launch in order: running loads in shared memory, the running Σ load() over healthy
+// workers and the threshold (Σ + 1) as f64 / n × load_factor in the operation order of prefix_fleet_prepare_kernel, the first healthy argmin
+// (looked for again only after it was picked).  load_ok is monotone in the load, so "least loaded worker passing load_ok" is that argmin when
+// it passes and none otherwise.  Loads start from `run` when from_run (a previous launch of the same call) and are left in `run` if non-null.
+__global__ void __launch_bounds__(32) prefix_feedback_kernel(const PrefixFleetView fleet, const __grid_constant__ PrefixArgs a, double load_factor,
+                                                             uint64_t* __restrict__ run, uint32_t from_run) {
+    extern __shared__ uint64_t s_L[];   // [n_slice]
+    const int lane = threadIdx.x;
+    const uint32_t ns = fleet.n_slice;
+    uint64_t total = 0;
+    for (uint32_t i = lane; i < ns; i += 32) {
+        const uint64_t l = from_run ? run[i] : fleet.loads[i];
+        s_L[i] = l;
+        if (fleet.flags[i] & 1) total += l;
+    }
+    for (int m = 16; m; m >>= 1) total += __shfl_xor_sync(0xFFFFFFFFu, total, m);
+    __syncwarp();
+    const uint32_t nh = fleet.derived->n_healthy;
+    auto least = [&]() {   // first argmin load over healthy workers (min_by_key → FIRST minimum)
+        uint64_t bl = 0; int32_t bi = -1;
+        for (uint32_t i = lane; i < ns; i += 32) if (fleet.flags[i] & 1) take_min(bl, bi, s_L[i], (int32_t)i);
+        for (int m = 16; m; m >>= 1) {
+            const uint64_t ol = __shfl_xor_sync(0xFFFFFFFFu, bl, m);
+            const int32_t oi = __shfl_xor_sync(0xFFFFFFFFu, bi, m);
+            take_min(bl, bi, ol, oi);
+        }
+        return bi;
+    };
+    int32_t hidx = least();
+    for (uint32_t j = 0; j < a.count; ++j) {
+        const PrefixBatch& bt = a.b[j];
+        if (!bt.out_idx) continue;
+        for (uint32_t r = 0; r < bt.n; ++r) {
+            const int64_t cand = (int64_t)bt.hash[r];
+            if (cand == kPhDecided) continue;
+            const bool all_ok = total == 0 || nh == 0;                                   // :117-119
+            const double thr = nh ? __dmul_rn(__ddiv_rn((double)(total + 1), (double)nh), load_factor) : 0.0;
+            int32_t idx;
+            uint8_t branch;
+            if (cand >= 0) {
+                const int32_t c = (int32_t)cand;
+                if (all_ok || (double)s_L[c] <= thr) { idx = c; branch = SMGX_PH_RING_HIT; }
+                else { idx = (hidx >= 0 && (double)s_L[hidx] <= thr) ? hidx : c; branch = SMGX_PH_LOAD_BALANCE_WALK; }
+            } else { idx = hidx; branch = SMGX_PH_FALLBACK_LEAST_LOAD; }
+            if (lane == 0) {
+                bt.out_idx[r] = idx;
+                if (bt.out_info) {
+                    smgx_decision_info o;
+                    o.matched = 0; o.input = __ldg(bt.offsets + r + 1) - __ldg(bt.offsets + r); o.branch = branch; o.nodes = 0;
+                    o.reserved[0] = o.reserved[1] = 0;
+                    bt.out_info[r] = o;
+                }
+            }
+            if (idx < 0) continue;
+            const uint64_t old = s_L[idx];   // the guard: load() + 1 on the pick (a healthy worker, so Σ grows too)
+            __syncwarp();
+            if (lane == 0) s_L[idx] = old + 1;
+            __syncwarp();
+            total += 1;
+            if (idx == hidx) hidx = least();
+        }
+    }
+    if (run) for (uint32_t i = lane; i < ns; i += 32) run[i] = s_L[i];
 }
 
 __global__ void __launch_bounds__(256) prefix_fleet_prepare_kernel(const uint64_t* __restrict__ loads, const uint8_t* __restrict__ flags, uint32_t n_slice,
@@ -282,7 +381,7 @@ void launch_prefix_fleet_prepare(const uint64_t* d_loads, const uint8_t* d_flags
 }
 
 uint32_t launch_prefix_select(const RingView& ring, const PrefixFleetView& fleet, const PrefixArgs& a, cudaStream_t stream, cudaStream_t pick_stream,
-                              cudaEvent_t hashes_ready) {
+                              cudaEvent_t hashes_ready, const PrefixFeedback* fb) {
     uint32_t max_n = 0;
     for (uint32_t k = 0; k < a.count; ++k) max_n = max_n > a.b[k].n ? max_n : a.b[k].n;
     if (max_n == 0 || a.count == 0) return 0;
@@ -294,10 +393,16 @@ uint32_t launch_prefix_select(const RingView& ring, const PrefixFleetView& fleet
             SMGX_CUDA(cudaEventRecord(hashes_ready, stream));
             SMGX_CUDA(cudaStreamWaitEvent(pick_stream, hashes_ready, 0));
         }
-        prefix_pick_kernel<<<dim3((max_n + kThreads - 1) / kThreads, a.count), kThreads, 0, pick_stream>>>(ring, fleet, a);
+        if (!fb) prefix_pick_kernel<<<dim3((max_n + kThreads - 1) / kThreads, a.count), kThreads, 0, pick_stream>>>(ring, fleet, a);
+        else {
+            const size_t smem = (size_t)(fleet.n_slice ? fleet.n_slice : 1) * 8;
+            if (smem > 48 * 1024) SMGX_CUDA(cudaFuncSetAttribute(prefix_feedback_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            prefix_candidate_kernel<<<dim3((max_n + kThreads - 1) / kThreads, a.count), kThreads, 0, pick_stream>>>(ring, fleet, a);
+            prefix_feedback_kernel<<<1, 32, smem, pick_stream>>>(fleet, a, fb->load_factor, fb->run_loads, fb->from_run);
+        }
     }
     SMGX_CUDA(cudaGetLastError());
-    return pick ? 2u : 1u;
+    return pick ? (fb ? 3u : 2u) : 1u;
 }
 
 void launch_ring_find(const uint64_t* d_ring_pos, const uint32_t* d_ring_url, uint32_t len, const uint64_t* d_key_pos, const uint8_t* d_url_ok, uint32_t n,

@@ -47,10 +47,15 @@ struct PrefixBatch {
 struct PrefixArgs { PrefixBatch b[kMaxPrefixBatches]; uint32_t count; uint32_t prefix_tokens; };
 
 void launch_prefix_fleet_prepare(const uint64_t* d_loads, const uint8_t* d_flags, uint32_t n_slice, double load_factor, PrefixDerived* d_out, cudaStream_t stream);
-// returns the number of kernels launched (1: hashes only, 2: hashes + picks)
-// pick_stream == stream: both kernels in order on one stream; otherwise the pick kernel is ordered after `hashes_ready` on pick_stream
+// Load feedback: the picks of a launch are made in request order on running loads (prefix_candidate_kernel + prefix_feedback_kernel instead
+// of prefix_pick_kernel).  run_loads (device, n_slice; nullable): the loads after the launch; from_run: start from them instead of the
+// snapshot (the next launch of the same call continues the stream).  The fleet must fit in shared memory: kMaxFeedbackSlice.
+struct PrefixFeedback { double load_factor; uint64_t* run_loads; uint32_t from_run; };
+constexpr uint32_t kMaxFeedbackSlice = 200 * 1024 / 8;
+// returns the number of kernels launched (1: hashes only, 2: hashes + picks, 3: hashes + the two load-feedback kernels)
+// pick_stream == stream: all kernels in order on one stream; otherwise the pick kernels are ordered after `hashes_ready` on pick_stream
 uint32_t launch_prefix_select(const RingView& ring, const PrefixFleetView& fleet, const PrefixArgs& a, cudaStream_t stream, cudaStream_t pick_stream,
-                              cudaEvent_t hashes_ready);
+                              cudaEvent_t hashes_ready, const PrefixFeedback* fb = nullptr);
 // HashRing::find_healthy_url for precomputed key positions and a per-ring-URL predicate; out[i] = ring URL index or -1
 void launch_ring_find(const uint64_t* d_ring_pos, const uint32_t* d_ring_url, uint32_t len, const uint64_t* d_key_pos, const uint8_t* d_url_ok, uint32_t n,
                       int32_t* d_out, cudaStream_t stream);

@@ -56,6 +56,7 @@ struct ModelState {
     std::string hash_arena_text;
     uint64_t hash_dead_tokens = 0, hash_dead_text = 0;   // arena elements / bytes no entry points at any more
     DevBuf d_slice_of_tenant;
+    std::vector<int32_t> slice_of_tenant;         // host copy of d_slice_of_tenant (the load-feedback decision of the tree modes)
     std::vector<uint32_t> tenant_of_slice;        // tenant id of urls[i]
     uint64_t seen_tenants_version = ~0ULL;
     bool has_learned_bs = false;
@@ -182,7 +183,7 @@ public:
                 if (pf_hash_ev[b]) cudaEventDestroy(pf_hash_ev[b]);
                 if (pf_pick_ev[b]) cudaEventDestroy(pf_pick_ev[b]);
             }
-            pf_stage.release(); pf_out.release();
+            pf_stage.release(); pf_out.release(); pf_run_loads.release();
             for (uint32_t q = 0; q < xch.peer.size(); ++q) if (q < xch.opened.size() && xch.opened[q] && xch.peer[q]) cudaIpcCloseMemHandle(xch.peer[q]);
             xch.local.release(); xch.d_bases.release(); xch.d_cand.release(); xch.d_fleet.release(); xch.d_arrive.release(); xch.d_gbase.release();
             d_err.release(); d_done_counters.release(); d_flush.release(); scratch.release(); scratch2.release(); d_gbase.release();
@@ -515,16 +516,76 @@ public:
         m.d_slice_of_tenant.reserve(sl.size() * 4);
         SMGX_CUDA(cudaMemcpyAsync(m.d_slice_of_tenant.ptr, sl.data(), sl.size() * 4, cudaMemcpyHostToDevice, ctrl));
         SMGX_CUDA(cudaStreamSynchronize(ctrl));
+        m.slice_of_tenant.swap(sl);
         m.fleet_dirty_tenant = false;
         m.seen_tenants_version = tenants.version;
     }
-    bool host_imbalanced(const ModelState& m) const {   // same f32 test as fleet_prepare_kernel (cache_aware.rs:669-670); used for mode dispatch only
-        if (m.loads.empty()) return false;
-        uint64_t mn = ~0ULL, mx = 0;
-        for (uint64_t l : m.loads) { mn = std::min(mn, l); mx = std::max(mx, l); }
+    // the f32 imbalance gate of fleet_prepare_kernel (cache_aware.rs:669-670): round-to-nearest conversions, an f32 product, strict >
+    bool imbalanced_f32(uint64_t mn, uint64_t mx) const {
         volatile float fmax = (float)mx;
         volatile float fprod = (float)mn * cfg.balance_rel_threshold;
         return (mx - mn) > cfg.balance_abs_threshold && fmax > fprod;
+    }
+    bool host_imbalanced(const ModelState& m) const {   // used for mode dispatch only
+        if (m.loads.empty()) return false;
+        uint64_t mn = ~0ULL, mx = 0;
+        for (uint64_t l : m.loads) { mn = std::min(mn, l); mx = std::max(mx, l); }
+        return imbalanced_f32(mn, mx);
+    }
+
+    // The fleet a tree-mode load-feedback batch runs against: the snapshot loads plus one per pick so far (the router's WorkerLoadGuard,
+    // routers/http/router.rs:319-321).  Kept as feedback_resolve_kernel keeps it: min / max over ALL workers (cache_aware.rs:662-666) with
+    // the number of workers at the minimum, and the first argmin over healthy workers with an ok circuit (min_by_key → FIRST minimum),
+    // looked for again only after it was itself picked.  The tree modes decide on the host, in the in-order pass that already commits
+    // every request's side effects, so a bump costs no launch.
+    struct RunningFleet {
+        std::vector<uint64_t> load;
+        const uint8_t* flags;
+        uint64_t gmin = ~0ULL, gmax = 0;
+        uint32_t at_gmin = 0;
+        int32_t hidx = -1, first_healthy = -1;
+        explicit RunningFleet(const ModelState& m) : load(m.loads), flags(m.flags.data()) {
+            for (size_t i = 0; i < load.size(); ++i) {
+                gmin = std::min(gmin, load[i]);
+                gmax = std::max(gmax, load[i]);
+                if (first_healthy < 0 && (flags[i] & 3) == 3) first_healthy = (int32_t)i;
+            }
+            if (load.empty()) gmin = 0;
+            for (uint64_t l : load) at_gmin += l == gmin;
+            rescan();
+        }
+        void rescan() {
+            hidx = -1;
+            for (size_t i = 0; i < load.size(); ++i)
+                if ((flags[i] & 3) == 3 && (hidx < 0 || load[i] < load[(size_t)hidx])) hidx = (int32_t)i;
+        }
+        void bump(int32_t w) {
+            const uint64_t old = load[(size_t)w]++;
+            gmax = std::max(gmax, old + 1);
+            if (old == gmin && --at_gmin == 0) { ++gmin; for (uint64_t l : load) at_gmin += l == gmin; }
+            if (w != hidx) return;
+            // workers before hidx are above the old minimum: the next argmin is a later worker still at it, or else found by a rescan
+            for (size_t i = (size_t)w + 1; i < load.size(); ++i)
+                if ((flags[i] & 3) == 3 && load[i] == old) { hidx = (int32_t)i; return; }
+            rescan();
+        }
+    };
+    // select_worker's load-dependent decision for one walked request against the running fleet (SURVEY Appendix A.1 steps 3, 4, 6/7):
+    // gate open → the first healthy argmin (select_worker_min_load); match rate above the threshold → the tenant's first slice position if
+    // is_healthy(), else healthy[0] (:892-894); otherwise the first healthy argmin.  Same f32 arithmetic as tree_walk_request.
+    void decide_running(const ModelState& m, const RunningFleet& rf, uint32_t matched, uint32_t input, int32_t tenant, int32_t* out,
+                        uint8_t* branch) const {
+        if (imbalanced_f32(rf.gmin, rf.gmax)) { *out = rf.hidx; *branch = SMGX_BR_IMBALANCED_MIN_LOAD; return; }
+        volatile float rate = input == 0 ? 0.0f : (float)matched / (float)input;
+        if (rate > cfg.cache_threshold) {
+            const int32_t sl = (tenant >= 0 && (size_t)tenant < m.slice_of_tenant.size()) ? m.slice_of_tenant[(size_t)tenant] : -1;
+            if (sl >= 0 && (m.flags[(size_t)sl] & 1)) { *out = sl; *branch = SMGX_BR_TREE_MATCH; }
+            else { *out = rf.first_healthy; *branch = SMGX_BR_TREE_FALLBACK_FIRST_HEALTHY; }
+        } else { *out = rf.hidx; *branch = SMGX_BR_TREE_MIN_LOAD; }
+    }
+    void refuse_snapshot_feedback() const {
+        if (tree_feedback && tree_batch_mode == SMGX_TREE_BATCH_SNAPSHOT)
+            throw Error(SMGX_INVALID_ARGUMENT, "cache_aware load feedback does not combine with SMGX_TREE_BATCH_SNAPSHOT (use SEQUENTIAL)");
     }
 
     // Approximate-token-tree mode (cache_aware.rs:834-904) and the imbalanced path's tree update (:380-402).
@@ -542,6 +603,7 @@ public:
         TokenTreeIndex& tree = tree_of(m, true);
         Lane& lane = use_lane ? *use_lane : lanes[0];
         if (forced) decide = false;
+        if (decide) refuse_snapshot_feedback();
         const uint64_t base = n ? offsets[0] : 0, total = n ? offsets[n] - base : 0;
         const uint32_t n1 = std::max<uint32_t>(n, 1);
         lane.d_tokens.reserve(std::max<uint64_t>(total, 1) * 4 + 16);
@@ -565,6 +627,10 @@ public:
         // requests in order and stops at the first one whose snapshot walk is no longer what a walk at that moment would
         // return — a path node was split, the node the walk stopped under gained a child for the next page, or (when the pick
         // used it) the deepest node's tenant changed.  Everything before it is committed; the walk restarts from there.
+        // Load feedback: the kernel's decision read the snapshot loads; each request is decided again here, in order, against the running
+        // fleet, which carries the committed prefix's bumps across restarts.
+        std::unique_ptr<RunningFleet> rf;
+        if (decide && tree_feedback) rf = std::make_unique<RunningFleet>(m);
         uint32_t seg = 0;
         while (seg < n) {
             const uint32_t end = n;
@@ -601,12 +667,15 @@ public:
                 const uint32_t* tk = tokens + offsets[r];
                 const uint32_t len = offsets[r + 1] - offsets[r];
                 if (decide && info[r].branch == SMGX_BR_NO_HEALTHY) continue;   // returns None before touching anything (:653-655)
+                int32_t pick = out_idx[r];
+                uint8_t pick_br = info[r].branch;
+                if (rf) decide_running(m, *rf, info[r].matched, info[r].input, ten[r], &pick, &pick_br);
                 const uint32_t* pth = path.data() + (size_t)r * kPathCap;
                 if (!snapshot && r > seg) {   // is the snapshot walk still the walk the reference would do now?
                     bool valid = path_len[r] <= kPathCap;
                     uint64_t sum_len = 0;
                     for (uint32_t d = 0; valid && d < path_len[r]; ++d) { valid = !tree.split_in_chunk(pth[d]); sum_len += tree.label_len_of(pth[d]); }
-                    const uint8_t br = info[r].branch;
+                    const uint8_t br = pick_br;
                     if (valid && path_len[r] && (br == SMGX_BR_TREE_MATCH || br == SMGX_BR_TREE_FALLBACK_FIRST_HEALTHY))
                         valid = tree.any_tenant(pth[path_len[r] - 1]) == ten[r];                       // the pick read this tenant
                     const uint32_t aligned = (len / kPage) * kPage;
@@ -628,6 +697,10 @@ public:
                     continue;
                 }
                 if (!decide) continue;
+                if (rf) {
+                    out_idx[r] = pick; info[r].branch = pick_br;
+                    if (pick >= 0) rf->bump(pick);   // WorkerLoadGuard on whatever select_worker returned, healthy[0] included
+                }
                 const uint8_t br = info[r].branch;
                 if ((br == SMGX_BR_TREE_MATCH || br == SMGX_BR_TREE_MIN_LOAD || br == SMGX_BR_IMBALANCED_MIN_LOAD) && out_idx[r] >= 0) {
                     const size_t idx = (size_t)out_idx[r];
@@ -774,6 +847,7 @@ public:
     // power_of_two policy (policies/power_of_two.rs:22): cached_loads, reduced to what select_worker reads — effective_token_usage() per URL
     std::unordered_map<std::string, double> p2c_usage;
     DevBuf pf_hash_buf[2];               // prefix hashes between the hash and pick kernels of the device-resident path
+    DevBuf pf_run_loads;                 // load feedback: running loads carried from one launch of a device-resident call to the next
     cudaEvent_t pf_hash_ev[2] = {nullptr, nullptr}, pf_pick_ev[2] = {nullptr, nullptr};
     bool pf_pick_pending[2] = {false, false};
     uint64_t pf_group = 0;
@@ -791,6 +865,7 @@ public:
     // start with the same char under the root (they then share a subtree) or when both end on the root itself.
     void text_select(ModelState& m, const uint8_t* text, const uint32_t* offsets, uint32_t n, int32_t* out_idx, smgx_decision_info* out_info,
                      bool decide, int32_t* out_tenant) {
+        if (decide) refuse_snapshot_feedback();
         StringTreeIndex& tree = stree_of(m);
         Lane& lane = lanes[0];
         const uint64_t base = n ? offsets[0] : 0, total = n ? offsets[n] - base : 0;
@@ -812,6 +887,8 @@ public:
         std::vector<uint64_t> path_hash;   // hash_node_path of every request (:950-956, :420-424)
         if (decide) enqueue_path_hashes(lane, lane.d_text.as<uint8_t>() - base, lane.d_offsets.as<uint32_t>(), offsets, n, 1, path_hash);
         const bool snapshot = tree_batch_mode == SMGX_TREE_BATCH_SNAPSHOT;
+        std::unique_ptr<RunningFleet> rf;   // load feedback, as in tree_select
+        if (decide && tree_feedback) rf = std::make_unique<RunningFleet>(m);
         uint32_t seg = 0;
         while (seg < n) {   // SEQUENTIAL runs optimistically, as in tree_select
             const uint32_t end = n;
@@ -839,11 +916,14 @@ public:
             uint32_t r = seg;
             for (; r < end; ++r) {
                 if (decide && info[r].branch == SMGX_BR_NO_HEALTHY) continue;
+                int32_t pick = out_idx[r];
+                uint8_t pick_br = info[r].branch;
+                if (rf) decide_running(m, *rf, info[r].matched, info[r].input, ten[r], &pick, &pick_br);
                 if (!snapshot && r > seg) {   // is the snapshot walk still the walk the reference would do now?
                     bool valid = true;
                     uint64_t sum_chars = 0;
                     for (uint32_t nd = node[r]; valid && nd != 0 && nd != kNoNode; nd = tree.parent_of(nd)) { valid = !tree.split_in_chunk(nd); sum_chars += tree.label_chars_of(nd); }
-                    const uint8_t br = info[r].branch;
+                    const uint8_t br = pick_br;
                     if (valid && (br == SMGX_BR_TREE_MATCH || br == SMGX_BR_TREE_FALLBACK_FIRST_HEALTHY)) valid = tree.any_tenant_of(node[r]) == ten[r];
                     if (valid && sum_chars == info[r].matched && info[r].matched < info[r].input) {   // stopped under a node: still no child for the next char?
                         const uint8_t* tx = text + offsets[r];
@@ -859,6 +939,10 @@ public:
                 if (snapshot) tree.apply_match_effects(node[r], ten[r], fill[r] != 0);
                 else tree.apply_match_effects(node[r], tree.any_tenant_of(node[r]), !tree.cache_valid_of(node[r]));
                 if (!decide) continue;
+                if (rf) {
+                    out_idx[r] = pick; info[r].branch = pick_br;
+                    if (pick >= 0) rf->bump(pick);
+                }
                 const uint8_t br = info[r].branch;
                 if ((br == SMGX_BR_TREE_MATCH || br == SMGX_BR_TREE_MIN_LOAD || br == SMGX_BR_IMBALANCED_MIN_LOAD) && out_idx[r] >= 0) {
                     const size_t idx = (size_t)out_idx[r];
@@ -1018,7 +1102,10 @@ public:
     uint64_t token_ts = 0;       // GLOBAL_TIMESTAMP (token_tree.rs:179), shared by every token tree of the policy
     uint64_t string_epoch = 0;   // EPOCH_COUNTER (string_tree.rs:239), shared by every string tree of the policy
     uint32_t tree_batch_mode = SMGX_TREE_BATCH_SEQUENTIAL;
-    bool load_feedback = false;   // smgx_set_load_feedback
+    bool load_feedback = false;   // event-driven calls as a request stream (smgx_set_load_feedback, or the CACHE_AWARE bit)
+    bool tree_feedback = false;   // token-tree / string-tree calls as a request stream (the CACHE_AWARE bit of smgx_set_load_feedback_policies)
+    bool prefix_feedback = false; // prefix_hash calls as a request stream (SMGX_FEEDBACK_PREFIX_HASH)
+    bool p2c_feedback = false;    // power_of_two calls as a request stream (SMGX_FEEDBACK_POWER_OF_TWO)
     uint32_t walk_chunk_seq = 0;
     smgx_cache_aware_config cfg;
     int sm_count = 132;              // H100 SXM; replaced by the device's own count when a device is opened
@@ -1845,7 +1932,8 @@ static smgx_status select_batch_text_once(smgx_policy* p, const char* model_key,
             if (toff[n]) SMGX_CUDA(cudaMemcpy(toks.data(), lane.d_tokens.ptr, (size_t)toff[n] * 4, cudaMemcpyDeviceToHost));
             if (out_tok_offsets) memcpy(out_tok_offsets, toff.data(), ((size_t)n + 1) * 4);
             if (out_tokens) { SMGX_REQUIRE(toff[n] <= cap_tokens, "token output buffer too small"); memcpy(out_tokens, toks.data(), (size_t)toff[n] * 4); }
-            P.tree_select(m, toks.data(), toff.data(), n, out_worker_idx, out_info, true, nullptr);
+            if (P.tree_feedback && P.has_event_indexer(m)) P.wait(P.submit_host(m, toks.data(), toff.data(), n, out_worker_idx, out_info));   // the gate is per request: the event-driven stream
+            else P.tree_select(m, toks.data(), toff.data(), n, out_worker_idx, out_info, true, nullptr);
             return SMGX_SUCCESS;
         }
         lane.d_out.reserve((size_t)n * 4);
@@ -2289,7 +2377,10 @@ static smgx_status prefix_host_call(smgx_policy* p, const char* model_key, const
         a.b[0].out_info = out_info ? lane.d_info.as<smgx_decision_info>() : nullptr;
         a.b[0].hash = lane.d_hashes.as<uint64_t>();
         a.b[0].n = n;
-        P.launches += launch_prefix_select(rv, fv, a, lane.stream, lane.stream, nullptr);
+        const bool fb = P.prefix_feedback && out_idx;
+        if (fb) SMGX_REQUIRE(fv.n_slice <= kMaxFeedbackSlice, "fleet too large for the load-feedback pass");
+        const PrefixFeedback pfb{P.prefix_load_factor, nullptr, 0};
+        P.launches += launch_prefix_select(rv, fv, a, lane.stream, lane.stream, nullptr, fb ? &pfb : nullptr);
         const size_t hash_at = ((size_t)n * (4 + sizeof(smgx_decision_info)) + 7) & ~(size_t)7;
         P.pf_out.reserve(hash_at + (size_t)n * 8);
         int32_t* h_idx = P.pf_out.as<int32_t>();
@@ -2333,6 +2424,12 @@ smgx_status smgx_prefix_hash_select_many_tokens_device(smgx_policy* p, const cha
         // the pick that read it has finished (event wait on lane 0).
         Lane& lane = P.lanes[0];
         Lane& side = P.lanes.size() > 1 ? P.lanes[1] : P.lanes[0];
+        // load feedback: every group's pick kernels run on `side` in order, each continuing from the running loads the previous one left
+        const bool fb = P.prefix_feedback;
+        if (fb) {
+            SMGX_REQUIRE(fv.n_slice <= kMaxFeedbackSlice, "fleet too large for the load-feedback pass");
+            if ((size_t)std::max<uint32_t>(fv.n_slice, 1) * 8 > P.pf_run_loads.cap) { SMGX_CUDA(cudaDeviceSynchronize()); P.pf_run_loads.reserve((size_t)std::max<uint32_t>(fv.n_slice, 1) * 8); }
+        }
         for (uint32_t j0 = 0; j0 < n_batches; j0 += kMaxPrefixBatches) {
             PrefixArgs a;
             a.count = std::min<uint32_t>(kMaxPrefixBatches, n_batches - j0);
@@ -2348,7 +2445,8 @@ smgx_status smgx_prefix_hash_select_many_tokens_device(smgx_policy* p, const cha
                 a.b[k] = PrefixBatch{d_tokens[j0 + k], d_offsets[j0 + k], nullptr, d_out_worker_idx[j0 + k], nullptr, P.pf_hash_buf[b].as<uint64_t>() + at, n[j0 + k]};
                 at += n[j0 + k];
             }
-            P.launches += launch_prefix_select(rv, fv, a, lane.stream, side.stream, P.pf_hash_ev[b]);
+            const PrefixFeedback pfb{P.prefix_load_factor, P.pf_run_loads.as<uint64_t>(), j0 > 0 ? 1u : 0u};
+            P.launches += launch_prefix_select(rv, fv, a, lane.stream, side.stream, P.pf_hash_ev[b], fb ? &pfb : nullptr);
             if (&side != &lane) { SMGX_CUDA(cudaEventRecord(P.pf_pick_ev[b], side.stream)); P.pf_pick_pending[b] = true; }
         }
         return SMGX_SUCCESS;
@@ -2446,7 +2544,8 @@ smgx_status smgx_submit_text(smgx_policy* p, const char* model_key, const uint8_
             SMGX_CUDA(cudaStreamSynchronize(lane.stream));
             std::vector<uint32_t> toks(std::max<uint32_t>(toff[n], 1));
             if (toff[n]) SMGX_CUDA(cudaMemcpy(toks.data(), lane.d_tokens.ptr, (size_t)toff[n] * 4, cudaMemcpyDeviceToHost));
-            P.tree_select(m, toks.data(), toff.data(), n, out_worker_idx, out_info, true, nullptr);
+            if (P.tree_feedback && P.has_event_indexer(m)) P.wait(P.submit_host(m, toks.data(), toff.data(), n, out_worker_idx, out_info));   // as in smgx_select_batch_text
+            else P.tree_select(m, toks.data(), toff.data(), n, out_worker_idx, out_info, true, nullptr);
             Lane& l2 = P.free_lane();
             l2.busy = true; l2.ticket = ++P.ticket_seq; l2.model = &m; l2.host_out = out_worker_idx; l2.n = 0;   // processed already counted
             *out_ticket = l2.ticket;
@@ -2507,6 +2606,22 @@ smgx_status smgx_set_load_feedback(smgx_policy* p, int enabled, char** err) {
         NONNULL(p);
         std::lock_guard<std::mutex> g(p->impl.mu);
         p->impl.load_feedback = enabled != 0;
+        p->impl.tree_feedback = p->impl.prefix_feedback = p->impl.p2c_feedback = false;
+        return SMGX_SUCCESS;
+    });
+}
+smgx_status smgx_set_load_feedback_policies(smgx_policy* p, uint32_t mask, char** err) {
+    return guard(err, [&]() {
+        NONNULL(p);
+        SMGX_REQUIRE((mask & ~(SMGX_FEEDBACK_CACHE_AWARE | SMGX_FEEDBACK_PREFIX_HASH | SMGX_FEEDBACK_POWER_OF_TWO)) == 0, "unknown load-feedback policy bit");
+        std::lock_guard<std::mutex> g(p->impl.mu);
+        const bool ca = (mask & SMGX_FEEDBACK_CACHE_AWARE) != 0;
+        SMGX_REQUIRE(!(ca && p->impl.tree_batch_mode == SMGX_TREE_BATCH_SNAPSHOT),
+                     "cache_aware load feedback does not combine with SMGX_TREE_BATCH_SNAPSHOT (use SEQUENTIAL)");
+        p->impl.load_feedback = ca;
+        p->impl.tree_feedback = ca;
+        p->impl.prefix_feedback = (mask & SMGX_FEEDBACK_PREFIX_HASH) != 0;
+        p->impl.p2c_feedback = (mask & SMGX_FEEDBACK_POWER_OF_TWO) != 0;
         return SMGX_SUCCESS;
     });
 }
@@ -2915,6 +3030,11 @@ smgx_status smgx_power_of_two_select_batch(smgx_policy* p, const char* model_key
         a.out_metric = reinterpret_cast<uint8_t*>(a.out_idx + n);
         launch_power_of_two(a, lane.stream);
         ++P.launches;
+        if (P.p2c_feedback) {
+            SMGX_REQUIRE(ns <= kMaxP2cFeedbackSlice, "fleet too large for the load-feedback pass");
+            launch_power_of_two_feedback(a, ns, lane.stream);
+            ++P.launches;
+        }
         SMGX_CUDA(cudaMemcpyAsync(out_worker_idx, a.out_idx, (size_t)n * 4, cudaMemcpyDeviceToHost, lane.stream));
         if (out_pairs) SMGX_CUDA(cudaMemcpyAsync(out_pairs, a.out_pair, (size_t)n * 8, cudaMemcpyDeviceToHost, lane.stream));
         if (out_metric) SMGX_CUDA(cudaMemcpyAsync(out_metric, a.out_metric, n, cudaMemcpyDeviceToHost, lane.stream));

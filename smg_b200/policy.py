@@ -875,6 +875,13 @@ class CacheAwarePolicy:
         (WorkerLoadGuard, routers/http/router.rs:319-321); off = one frozen fleet snapshot per batch."""
         self._h.call("smgx_set_load_feedback", 1 if enabled else 0)
 
+    def set_load_feedback_all_modes(self, enabled: bool):
+        """Every cache_aware mode as a request STREAM (SMGX_FEEDBACK_CACHE_AWARE): the event-driven calls as set_load_feedback(True) does,
+        and the token-tree and string-tree calls, whose imbalance gate, min-load picks and healthy[0] fallback then read the snapshot loads
+        plus one per earlier pick of the call.  Refused in the "snapshot" tree batch mode.  This and set_load_feedback set one state: the
+        last call wins."""
+        self._h.call("smgx_set_load_feedback_policies", 1 if enabled else 0)
+
     def set_tree_batch_mode(self, mode: str):
         self._h.call("smgx_set_tree_batch_mode", TREE_BATCH_MODES[mode])
 
@@ -991,6 +998,12 @@ class PrefixHashPolicy:
         self._h.call("smgx_prefix_hash_configure", int(self.config.prefix_token_count), float(self.config.load_factor))
         self._slices = {}
         self._ring_of = {}
+
+    def set_load_feedback(self, enabled: bool):
+        """Batches as the request stream of a router that guards every pick (the gRPC router, routers/grpc/context.rs:248-259): request i
+        sees the snapshot loads plus one per pick of requests < i, in the bound (Σ load + 1) / n × load_factor and the least loaded fallback.
+        Every batch of one device-resident call forms one stream.  Off = one frozen fleet snapshot per batch."""
+        self._h.call("smgx_set_load_feedback_policies", 2 if enabled else 0)
 
     @classmethod
     def with_defaults(cls, **kw):  # :100-103
@@ -1124,6 +1137,11 @@ class PowerOfTwoPolicy:
         circuit = np.ascontiguousarray(np.asarray([1 if w.circuit_breaker_can_execute() else 0 for w in workers] or [0], dtype=np.uint8))
         self._h.call("smgx_set_fleet_state", model, _p(loads) if len(workers) else None, _p(healthy), _p(circuit), len(workers))
         return model
+
+    def set_load_feedback(self, enabled: bool):
+        """Batches as the request stream of a router that guards every pick (the gRPC router, routers/grpc/context.rs:248-259): the draws
+        and pairs are unchanged, the request-count comparison reads the snapshot loads plus one per pick of requests < i."""
+        self._h.call("smgx_set_load_feedback_policies", 4 if enabled else 0)
 
     def next_seed(self) -> int:
         self._calls += 1
