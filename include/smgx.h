@@ -323,6 +323,33 @@ smgx_status smgx_prefix_hash_select_batch_tokens(smgx_policy* p, const char* mod
 smgx_status smgx_prefix_hash_select_many_tokens_device(smgx_policy* p, const char* model_key, uint32_t n_batches, const uint32_t* const* d_tokens,
                                                        const uint32_t* const* d_offsets, const uint32_t* n, int32_t* const* d_out_worker_idx, char** err);
 
+/* ---- adjacent policy on the same plumbing: consistent_hashing (model_gateway/src/policies/consistent_hashing.rs) ---- */
+/* Which branch of ConsistentHashingPolicy::select_worker_impl produced the result, in Branch::as_str order (:31-51). */
+typedef enum smgx_ch_branch {
+    SMGX_CH_NO_HEALTHY_WORKERS = 0,   /* empty slice, no healthy worker for the key, or no healthy worker for the random pick */
+    SMGX_CH_TARGET_WORKER_HIT = 1,    /* X-SMG-Target-Worker names a healthy slice index (:128-137)                           */
+    SMGX_CH_TARGET_WORKER_MISS = 2,   /* X-SMG-Target-Worker is not a usize, out of range or unhealthy → None                 */
+    SMGX_CH_ROUTING_KEY_HIT = 3,      /* X-SMG-Routing-Key, else the implicit authorization / x-forwarded-for / cookie key     */
+    SMGX_CH_RANDOM_FALLBACK = 4       /* no key: a uniformly drawn is_healthy() worker (:163-185)                              */
+} smgx_ch_branch;
+/* ConsistentHashingPolicy::select_worker_impl (:116-186) for n requests against the worker slice and fleet snapshot of `model_key`
+ * (smgx_set_workers + smgx_set_fleet_state; only is_healthy() is read, the circuit breaker is not) and the model's ring: the ring of
+ * smgx_hash_ring_set, none before it or after smgx_hash_ring_clear (info.hash_ring = None → the modulo fallback over the sorted healthy
+ * indices, one per URL).  Headers of request i: header h = values[offsets[5i+h] .. offsets[5i+h+1]) for h = 0 x-smg-target-worker,
+ * 1 x-smg-routing-key, 2 authorization, 3 x-forwarded-for, 4 cookie; present[i] bit h = HeaderMap::get(name h) returned Some (the first
+ * value of a repeated header; info.headers = None ⇔ 0).  A value is used only if every byte is \t or 0x20..=0x7E (HeaderValue::to_str)
+ * and it is non-empty; the target worker is parsed as usize::from_str.  The implicit key is the first PRESENT of authorization,
+ * x-forwarded-for, cookie, and an empty or non-visible value there goes to the random fallback.  The reference draws the random fallback
+ * from an unseedable thread-local generator; here request i uses draw i of the counter-based stream `seed` selects (the power_of_two
+ * stream), mapped to ⌊x·h / 2^64⌋ over the h healthy workers in slice order, so a caller advances `seed` per call.
+ * Host buffers; offsets (5n + 1, non-decreasing) need not start at 0 and only values[offsets[0] .. offsets[5n]) crosses PCIe.  Any present
+ * x-smg-routing-key, authorization, x-forwarded-for or cookie value longer than 2 MiB is SMGX_INVALID_ARGUMENT for the whole call, whether
+ * or not it would be the key used (the check runs on the offsets, before any byte is read); the target-worker value has no limit.  out_branch (n, nullable): smgx_ch_branch; out_key_pos (n, nullable): blake3(key)[..8] LE of
+ * the key used, 0 when no key was hashed.  No pick reads a load, so load feedback (smgx_set_load_feedback_policies) does not apply. */
+smgx_status smgx_consistent_hashing_select_batch(smgx_policy* p, const char* model_key, uint32_t n, const uint8_t* values, const uint32_t* offsets,
+                                                 const uint8_t* present, uint64_t seed, int32_t* out_worker_idx, uint8_t* out_branch,
+                                                 uint64_t* out_key_pos, char** err);
+
 /* ---- HTTP text routing: select_worker with info.request_text = Some(text), info.tokens = None ------------------ */
 /* select_worker_with_text (cache_aware.rs:907-974) and the imbalanced path's string-tree update (:403-425) for a batch:
  * request i = text[offsets[i] .. offsets[i+1]) (valid UTF-8).  match_rate = matched chars / input chars (f32, strict >).

@@ -10,13 +10,16 @@
 //   kv_index::PositionalIndexer        crates/kv_index/src/event_tree.rs:257-444     → smgx::PositionalIndexer
 //   worker::KvEventMonitor (the slice the policy reads + apply_event)                 → smgx::KvEventMonitor
 //   struct PrefixHashPolicy / HashRing  policies/prefix_hash.rs:87-235, worker/hash_ring.rs:29-150 → smgx::PrefixHashPolicy / smgx::HashRing
+//   struct ConsistentHashingPolicy      policies/consistent_hashing.rs:53-196       → smgx::ConsistentHashingPolicy
 // Header-only; link with -lsmgx.  All work happens in the library's CUDA kernels — there is no CPU fallback behind these classes.
 #pragma once
+#include <cctype>
 #include <cstdint>
 #include <cstring>
 #include <map>
 #include <memory>
 #include <optional>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -67,10 +70,14 @@ struct CacheAwareConfig {   // policies/mod.rs:94-117 (+Default)
 };
 
 class HashRing;
-struct SelectWorkerInfo {   // policies/mod.rs:161-175 (headers are not read on this path; hash_ring only by prefix_hash)
+// HeaderMap as (name, value) pairs in insertion order; names compare case-insensitively and get() returns the first value of a name
+using HeaderMap = std::vector<std::pair<std::string, std::string>>;
+
+struct SelectWorkerInfo {   // policies/mod.rs:161-175 (headers are read by consistent_hashing only; hash_ring by prefix_hash and consistent_hashing)
     std::optional<std::string> request_text;
     std::optional<std::vector<uint32_t>> tokens;
     std::shared_ptr<HashRing> hash_ring;
+    std::optional<HeaderMap> headers;
 };
 
 class Worker {   // the scalars CacheAwarePolicy reads through `trait Worker`
@@ -498,6 +505,79 @@ public:
 private:
     std::shared_ptr<detail::Handle> h_;
     std::map<std::string, std::vector<std::string>> slices_;
+    uint64_t seed_, calls_ = 0;
+};
+
+class ConsistentHashingPolicy : public LoadBalancingPolicy {   // consistent_hashing.rs:53-196
+public:
+    explicit ConsistentHashingPolicy(int device_id = 0, uint32_t max_batch = 0, uint64_t seed = 0x5EED) : seed_(seed) {
+        smgx_cache_aware_config c;
+        smgx_default_config(&c);
+        c.eviction_interval_secs = 0; c.device_id = device_id; c.max_batch = max_batch;
+        h_ = std::make_shared<detail::Handle>(c);
+    }
+    const char* name() const override { return "consistent_hashing"; }      // :188-190
+    // the registry's per-model ring, bound to this policy's device state
+    std::shared_ptr<HashRing> hash_ring(const std::vector<std::string>& urls, const std::string& model = "unknown") {
+        return std::make_shared<HashRing>(h_, normalize_model_key(model), urls);
+    }
+    struct Batch { std::vector<int32_t> idx; std::vector<uint8_t> branch; std::vector<uint64_t> key_pos; };   // branch: smgx_ch_branch
+    // one batch against one snapshot of the slice (headers[i] = std::nullopt: info.headers = None); every call consumes one value of the
+    // policy's seed sequence, request i uses draw i of it
+    Batch select_worker_batch(const Workers& workers, const std::vector<std::optional<HeaderMap>>& headers, const std::shared_ptr<HashRing>& ring = nullptr) {
+        static const char* const kNames[5] = {"x-smg-target-worker", "x-smg-routing-key", "authorization", "x-forwarded-for", "cookie"};
+        std::string model = ring ? ring->model() : normalize_model_key(workers.empty() ? "" : workers[0]->model_id());
+        if (ring && ring->handle() != h_) throw Error(SMGX_INVALID_ARGUMENT, "hash ring belongs to another policy: build it with ConsistentHashingPolicy::hash_ring()");
+        char* err = nullptr;
+        if (!ring && ringed_.count(model)) { detail::check(smgx_hash_ring_clear(h_->p, model.c_str(), &err), err); ringed_.erase(model); }
+        if (ring) ringed_.insert(model);
+        std::vector<std::string> urls;
+        for (auto& w : workers) urls.push_back(w->url());
+        auto it = slices_.find(model);
+        if (it == slices_.end() || it->second != urls) {
+            std::vector<const char*> c;
+            for (auto& u : urls) c.push_back(u.c_str());
+            detail::check(smgx_set_workers(h_->p, model.c_str(), c.data(), (uint32_t)c.size(), &err), err);
+            slices_[model] = urls;
+        }
+        std::vector<uint64_t> loads;
+        std::vector<uint8_t> healthy, circuit;
+        for (auto& w : workers) { loads.push_back(w->load()); healthy.push_back(w->is_healthy()); circuit.push_back(w->circuit_breaker_can_execute()); }
+        detail::check(smgx_set_fleet_state(h_->p, model.c_str(), loads.data(), healthy.data(), circuit.data(), (uint32_t)workers.size(), &err), err);
+        const uint32_t n = (uint32_t)headers.size();
+        std::string values;
+        std::vector<uint32_t> offsets{0};
+        std::vector<uint8_t> present(n, 0);
+        for (uint32_t i = 0; i < n; ++i)
+            for (int h = 0; h < 5; ++h) {
+                if (headers[i])
+                    for (auto& kv : *headers[i]) {
+                        if (!iequals(kv.first, kNames[h])) continue;
+                        present[i] |= (uint8_t)(1u << h); values += kv.second;
+                        break;
+                    }
+                offsets.push_back((uint32_t)values.size());
+            }
+        Batch b{std::vector<int32_t>(n, -1), std::vector<uint8_t>(n, 0), std::vector<uint64_t>(n, 0)};
+        ++calls_;
+        detail::check(smgx_consistent_hashing_select_batch(h_->p, model.c_str(), n, (const uint8_t*)values.data(), offsets.data(), present.data(),
+                                                           seed_ + 0xD1B54A32D192ED03ULL * calls_, b.idx.data(), b.branch.data(), b.key_pos.data(), &err), err);
+        return b;
+    }
+    std::pair<std::optional<size_t>, smgx_ch_branch> select_worker_impl(const Workers& workers, const SelectWorkerInfo& info) {   // :116-180
+        const Batch b = select_worker_batch(workers, {info.headers}, info.hash_ring);
+        return {b.idx[0] < 0 ? std::nullopt : std::optional<size_t>((size_t)b.idx[0]), (smgx_ch_branch)b.branch[0]};
+    }
+    std::optional<size_t> select_worker(const Workers& workers, const SelectWorkerInfo& info) override { return select_worker_impl(workers, info).first; }   // :182-186
+private:
+    static bool iequals(const std::string& a, const char* b) {
+        size_t i = 0;
+        for (; i < a.size() && b[i]; ++i) if (std::tolower((unsigned char)a[i]) != b[i]) return false;
+        return i == a.size() && !b[i];
+    }
+    std::shared_ptr<detail::Handle> h_;
+    std::map<std::string, std::vector<std::string>> slices_;
+    std::set<std::string> ringed_;
     uint64_t seed_, calls_ = 0;
 };
 

@@ -5,5 +5,6 @@ host-side mirror of the reference's plugin surface (policies::CacheAwarePolicy, 
 the parity tests and bench.py; it adds no logic of its own and has no CPU fallback.
 """
 from .policy import (BasicWorker, CacheAwareConfig, CacheAwarePolicy, KvEventMonitor, PositionalIndexer, SelectWorkerInfo,  # noqa: F401
-                     PolicyFactory, TiktokenTokenizer, HuggingFaceTokenizer, TokenTree, Tree, HashRing, PrefixHashConfig, PrefixHashPolicy, PowerOfTwoPolicy)
+                     PolicyFactory, TiktokenTokenizer, HuggingFaceTokenizer, TokenTree, Tree, HashRing, PrefixHashConfig, PrefixHashPolicy, PowerOfTwoPolicy,
+                     ConsistentHashingPolicy)
 from ._lib import SmgxError  # noqa: F401

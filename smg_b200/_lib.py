@@ -116,6 +116,7 @@ def load():
     sig("smgx_prefix_hash_configure", st, vp, u64, C.c_double, pp)
     sig("smgx_power_of_two_update_loads", st, vp, P(cp), vp, u32, pp)
     sig("smgx_power_of_two_select_batch", st, vp, cp, u32, u64, vp, vp, vp, pp)
+    sig("smgx_consistent_hashing_select_batch", st, vp, cp, u32, vp, vp, vp, u64, vp, vp, vp, pp)
     sig("smgx_hash_ring_set", st, vp, cp, P(cp), u32, pp)
     sig("smgx_hash_ring_clear", st, vp, cp, pp)
     sig("smgx_hash_ring_entries", st, vp, cp, vp, vp, u32, P(u32), pp)

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsmgx.so")
-SOURCES = ["smgx.cu", "event_index.cu", "event_kernels.cu", "tokenizer.cu", "token_tree.cu", "string_tree.cu", "blake3.cu", "prefix_hash.cu", "power_of_two.cu"]
+SOURCES = ["smgx.cu", "event_index.cu", "event_kernels.cu", "tokenizer.cu", "token_tree.cu", "string_tree.cu", "blake3.cu", "prefix_hash.cu", "power_of_two.cu", "consistent_hashing.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CFLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

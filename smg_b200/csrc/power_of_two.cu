@@ -9,16 +9,10 @@
 #include "power_of_two.h"
 
 #include "common.h"
+#include "counter_draw.cuh"
 
 namespace smgx {
 namespace {
-
-__device__ __forceinline__ uint64_t p2c_mix(uint64_t x) {
-    x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ULL;
-    x ^= x >> 27; x *= 0x94D049BB133111EBULL;
-    return x ^ (x >> 31);
-}
-__device__ __forceinline__ uint64_t p2c_draw(uint64_t seed, uint64_t k) { return p2c_mix(seed + 0x9E3779B97F4A7C15ULL * (k + 1)); }
 
 __global__ void __launch_bounds__(256) power_of_two_kernel(const P2cArgs a) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -10,6 +10,7 @@
 #include "prefix_hash.h"
 
 #include "blake3.cuh"
+#include "ring_walk.cuh"
 #include "xxh3.cuh"
 
 namespace smgx {
@@ -144,7 +145,6 @@ __global__ void __launch_bounds__(kHashThreads) prefix_hash_kernel(const __grid_
 // HashRing::find_healthy_url (hash_ring.rs:102-134) of a request's prefix hash over the slice's healthy workers: its ring candidate,
 // -1 when no ring URL resolves to a healthy slice entry.  Shared by the pick kernel and the load-feedback candidate kernel.
 __device__ __forceinline__ int32_t ring_candidate(const RingView& ring, const PrefixFleetView& fleet, uint64_t ph) {
-    int32_t initial = -1;
     // key = format!("{prefix_hash:016x}"): 16 lower-case hex digits, most significant first, as one blake3 block
     uint32_t m[16];
 #pragma unroll
@@ -163,21 +163,7 @@ __device__ __forceinline__ int32_t ring_candidate(const RingView& ring, const Pr
 #pragma unroll
     for (int q = 0; q < 8; ++q) cv[q] = b3::kIV[q];
     b3::compress(cv, m, 0, 16, b3::CHUNK_START | b3::CHUNK_END | b3::ROOT);
-    const uint64_t key_pos = mk64(cv[0], cv[1]);
-    // partition_point(|pos| pos < key_pos): positions are uniform 64-bit hashes, so a table of "first entry at or above
-    // bucket b's lower bound" (2+ buckets per entry) lands within an entry or two of the answer — two dependent loads, not 14
-    const uint32_t bk = (uint32_t)(key_pos >> ring.bucket_shift);
-    uint32_t lo = __ldg(ring.bucket + bk);
-    const uint32_t hi = __ldg(ring.bucket + bk + 1);
-    while (lo < hi && __ldg(ring.pos + lo) < key_pos) ++lo;
-    uint32_t e = lo == ring.len ? 0 : lo;
-    for (uint32_t step = 0; step < ring.len; ++step) {
-        int32_t s = __ldg(ring.slice + e);
-        while (s >= 0 && !(fleet.flags[s] & 1)) s = fleet.dup_prev[s];   // the URL resolves to its last HEALTHY slice entry
-        if (s >= 0) { initial = s; break; }
-        if (++e == ring.len) e = 0;
-    }
-    return initial;
+    return ring_walk(ring, fleet, mk64(cv[0], cv[1]));
 }
 
 // K-prefix-2: one thread per request: ring lookup + bounded-load pick from bt.hash[r]

@@ -25,6 +25,7 @@
 #include "blake3.h"
 #include "prefix_hash.h"
 #include "power_of_two.h"
+#include "consistent_hashing.h"
 #include <cstdio>
 #include <cctype>
 #include <sched.h>
@@ -76,6 +77,12 @@ struct ModelState {
     uint32_t ring_bucket_shift = 63;
     bool pf_struct_dirty = true;          // slice or ring changed: entry → slice map must be rebuilt
     bool pf_state_dirty = true;           // loads / health changed: fleet summary must be recomputed
+    // consistent_hashing policy (policies/consistent_hashing.rs): per fleet snapshot, the ascending is_healthy() indices followed by the
+    // ascending values of the healthy URL → last healthy index map
+    DevBuf d_ch_lists;
+    std::vector<int32_t> ch_lists;
+    uint32_t ch_n_healthy = 0;
+    bool ch_dirty = true;
 };
 
 struct Lane {
@@ -175,7 +182,7 @@ public:
                 m.string_tree.reset();
                 m.d_slice_of_tenant.release();
                 m.d_ring_pos.release(); m.d_ring_slice.release(); m.d_ring_url.release(); m.d_ring_bucket.release(); m.d_dup_prev.release();
-                m.d_pf_loads.release(); m.d_pf_flags.release(); m.d_pf_derived.release();
+                m.d_pf_loads.release(); m.d_pf_flags.release(); m.d_pf_derived.release(); m.d_ch_lists.release();
             }
             for (uint32_t i = 0; i < kPipeSlots; ++i) { if (pipe_hashed[i]) cudaEventDestroy(pipe_hashed[i]); if (pipe_searched[i]) cudaEventDestroy(pipe_searched[i]); }
             for (int b = 0; b < 2; ++b) {
@@ -183,7 +190,7 @@ public:
                 if (pf_hash_ev[b]) cudaEventDestroy(pf_hash_ev[b]);
                 if (pf_pick_ev[b]) cudaEventDestroy(pf_pick_ev[b]);
             }
-            pf_stage.release(); pf_out.release(); pf_run_loads.release();
+            pf_stage.release(); pf_out.release(); pf_run_loads.release(); ch_stage.release(); ch_out.release();
             for (uint32_t q = 0; q < xch.peer.size(); ++q) if (q < xch.opened.size() && xch.opened[q] && xch.peer[q]) cudaIpcCloseMemHandle(xch.peer[q]);
             xch.local.release(); xch.d_bases.release(); xch.d_cand.release(); xch.d_fleet.release(); xch.d_arrive.release(); xch.d_gbase.release();
             d_err.release(); d_done_counters.release(); d_flush.release(); scratch.release(); scratch2.release(); d_gbase.release();
@@ -835,12 +842,32 @@ public:
                                         lane.stream);
             ++launches;
             m.pf_state_dirty = false;
+            m.ch_dirty = true;
         }
         rv->pos = m.d_ring_pos.as<uint64_t>(); rv->slice = m.d_ring_slice.as<int32_t>(); rv->len = len; rv->has_ring = m.has_ring ? 1u : 0u;
         rv->bucket = m.d_ring_bucket.as<uint32_t>(); rv->bucket_shift = m.ring_bucket_shift;
         fv->loads = m.d_pf_loads.as<uint64_t>(); fv->flags = m.d_pf_flags.as<uint8_t>(); fv->dup_prev = m.d_dup_prev.as<int32_t>();
         fv->derived = m.d_pf_derived.as<PrefixDerived>(); fv->n_slice = ns;
     }
+    // ring and fleet views for consistent_hashing, with the two index lists of the current fleet snapshot (in lane-0 stream order)
+    void sync_chash(ModelState& m, RingView* rv, PrefixFleetView* fv) {
+        sync_prefix(m, rv, fv);
+        if (!m.ch_dirty) return;
+        const uint32_t ns = (uint32_t)m.urls.size();
+        m.ch_lists.clear();
+        std::unordered_map<std::string, int32_t> last_of;   // healthy_url_to_idx (consistent_hashing.rs:74-79): a later duplicate overwrites
+        for (uint32_t i = 0; i < ns; ++i)
+            if (m.flags[i] & 1) { m.ch_lists.push_back((int32_t)i); last_of[m.urls[i]] = (int32_t)i; }
+        m.ch_n_healthy = (uint32_t)m.ch_lists.size();
+        for (auto& kv : last_of) m.ch_lists.push_back(kv.second);
+        std::sort(m.ch_lists.begin() + m.ch_n_healthy, m.ch_lists.end());   // sort_unstable (:95)
+        m.d_ch_lists.reserve(std::max<size_t>(m.ch_lists.size(), 1) * 4);
+        Lane& lane = lanes[0];
+        if (!m.ch_lists.empty())
+            SMGX_CUDA(cudaMemcpyAsync(m.d_ch_lists.ptr, m.ch_lists.data(), m.ch_lists.size() * 4, cudaMemcpyHostToDevice, lane.stream));
+        m.ch_dirty = false;
+    }
+    PinBuf ch_stage, ch_out;             // pinned staging of the consistent_hashing call
     uint64_t prefix_token_count = 256;   // PrefixHashConfig::default() (prefix_hash.rs:52-58)
     double prefix_load_factor = 1.25;
     PinBuf pf_stage, pf_out;             // pinned staging of the host-buffer prefix_hash call
@@ -3039,6 +3066,72 @@ smgx_status smgx_power_of_two_select_batch(smgx_policy* p, const char* model_key
         if (out_pairs) SMGX_CUDA(cudaMemcpyAsync(out_pairs, a.out_pair, (size_t)n * 8, cudaMemcpyDeviceToHost, lane.stream));
         if (out_metric) SMGX_CUDA(cudaMemcpyAsync(out_metric, a.out_metric, n, cudaMemcpyDeviceToHost, lane.stream));
         SMGX_CUDA(cudaStreamSynchronize(lane.stream));
+        return SMGX_SUCCESS;
+    });
+}
+// ---- adjacent policy: consistent_hashing (model_gateway/src/policies/consistent_hashing.rs) ----
+smgx_status smgx_consistent_hashing_select_batch(smgx_policy* p, const char* model_key, uint32_t n, const uint8_t* values, const uint32_t* offsets,
+                                                 const uint8_t* present, uint64_t seed, int32_t* out_worker_idx, uint8_t* out_branch,
+                                                 uint64_t* out_key_pos, char** err) {
+    return guard(err, [&]() {
+        NONNULL(p);
+        SMGX_REQUIRE(n == 0 || (offsets && present && out_worker_idx), "Invalid arguments: null pointer");
+        SMGX_REQUIRE(n <= (0xFFFFFFFFu - 1) / kChashHeaders, "batch too large");
+        std::lock_guard<std::mutex> g(p->impl.mu);
+        Policy& P = p->impl;
+        P.use_device();
+        ModelState& m = P.model(model_key, false);
+        if (n == 0) return SMGX_SUCCESS;
+        const uint32_t ns = (uint32_t)m.urls.size();
+        SMGX_REQUIRE(m.loads.size() == ns && m.flags.size() == ns, "fleet state not set for this model (smgx_set_fleet_state)");
+        const uint32_t n_off = kChashHeaders * n + 1;
+        uint32_t max_long = 0;
+        for (uint32_t k = 0; k + 1 < n_off; ++k) {
+            SMGX_REQUIRE(offsets[k + 1] >= offsets[k], "offsets must be non-decreasing");
+            const uint32_t len = offsets[k + 1] - offsets[k], h = k % kChashHeaders;
+            if (h == 0 || !((present[k / kChashHeaders] >> h) & 1)) continue;   // only a routing key or an implicit key is hashed
+            SMGX_REQUIRE(len <= kChashMaxKeyBytes, "header value longer than 2 MiB");
+            if (len > 1024) ++max_long;
+        }
+        const uint32_t base = offsets[0], bytes = offsets[n_off - 1] - base;
+        SMGX_REQUIRE(bytes == 0 || values, "Invalid arguments: null pointer");
+        // one pinned staging area, one copy: values | offsets rebased to 0 | present
+        const size_t off_at = ((size_t)bytes + 15) & ~(size_t)15, pres_at = off_at + (size_t)n_off * 4;
+        P.ch_stage.reserve(pres_at + n + 16);
+        uint8_t* h_in = P.ch_stage.as<uint8_t>();
+        if (bytes) memcpy(h_in, values + base, bytes);
+        uint32_t* h_off = reinterpret_cast<uint32_t*>(h_in + off_at);
+        for (uint32_t k = 0; k < n_off; ++k) h_off[k] = offsets[k] - base;
+        memcpy(h_in + pres_at, present, n);
+        Lane& lane = P.lanes[0];
+        const size_t in_bytes = pres_at + n;
+        lane.d_text.reserve(in_bytes + 16);
+        SMGX_CUDA(cudaMemcpyAsync(lane.d_text.ptr, h_in, in_bytes, cudaMemcpyHostToDevice, lane.stream));
+        RingView rv; PrefixFleetView fv;
+        P.sync_chash(m, &rv, &fv);
+        // outputs: key_pos (8n) | idx (4n) | branch (n), then the long-key queue (12n) and its length
+        const size_t idx_at = (size_t)n * 8, br_at = idx_at + (size_t)n * 4, q_at = (br_at + n + 15) & ~(size_t)15;
+        const size_t qlen_at = q_at + (size_t)n * sizeof(ChashLongKey);
+        lane.d_out.reserve(qlen_at + 16);
+        uint8_t* d_out = lane.d_out.as<uint8_t>();
+        uint8_t* d_in = lane.d_text.as<uint8_t>();
+        ChashArgs a;
+        a.values = d_in; a.offsets = reinterpret_cast<const uint32_t*>(d_in + off_at); a.present = d_in + pres_at;
+        a.n = n; a.seed = seed; a.ring = rv; a.fleet = fv;
+        a.healthy = m.d_ch_lists.as<int32_t>(); a.n_healthy = m.ch_n_healthy;
+        a.url_last = a.healthy + m.ch_n_healthy; a.n_url_last = (uint32_t)m.ch_lists.size() - m.ch_n_healthy;
+        a.out_key_pos = reinterpret_cast<uint64_t*>(d_out); a.out_idx = reinterpret_cast<int32_t*>(d_out + idx_at); a.out_branch = d_out + br_at;
+        a.queue = reinterpret_cast<ChashLongKey*>(d_out + q_at); a.queue_len = reinterpret_cast<uint32_t*>(d_out + qlen_at);
+        P.launches += launch_consistent_hashing(a, max_long, P.sm_count, lane.stream);
+        const size_t out_bytes = out_key_pos ? br_at + n : (out_branch ? (size_t)n * 5 : (size_t)n * 4);
+        const size_t out_from = out_key_pos ? 0 : idx_at;
+        P.ch_out.reserve(br_at + n + 16);
+        uint8_t* h_out = P.ch_out.as<uint8_t>();
+        SMGX_CUDA(cudaMemcpyAsync(h_out + out_from, d_out + out_from, out_bytes, cudaMemcpyDeviceToHost, lane.stream));
+        SMGX_CUDA(cudaStreamSynchronize(lane.stream));
+        memcpy(out_worker_idx, h_out + idx_at, (size_t)n * 4);
+        if (out_branch) memcpy(out_branch, h_out + br_at, n);
+        if (out_key_pos) memcpy(out_key_pos, h_out, (size_t)n * 8);
         return SMGX_SUCCESS;
     });
 }

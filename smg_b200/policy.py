@@ -11,7 +11,7 @@ Every decision comes out of the CUDA kernels; this file only marshals arrays.
 """
 import ctypes as C
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import List, Mapping, Optional, Sequence
 
 import numpy as np
 
@@ -35,10 +35,11 @@ class CacheAwareConfig:  # policies/mod.rs:94-117
 
 
 @dataclass
-class SelectWorkerInfo:  # policies/mod.rs:161-175 (headers are not read on this path; hash_ring only by prefix_hash)
+class SelectWorkerInfo:  # policies/mod.rs:161-175 (headers are read by consistent_hashing only; hash_ring by prefix_hash and consistent_hashing)
     request_text: Optional[str] = None
     tokens: Optional[Sequence[int]] = None
     hash_ring: Optional["HashRing"] = None
+    headers: Optional[Mapping] = None   # header name (any case) → value (str or bytes, or a list whose first item HeaderMap::get returns)
 
 
 class BasicWorker:
@@ -989,6 +990,43 @@ class HashRing:
         return self.find_healthy_urls([key], is_healthy)[0]
 
 
+def _push_ring_fleet(policy, workers, ring: Optional[HashRing], with_circuit: bool) -> bytes:
+    """The slice, loads and is_healthy() of a ring-reading policy (policy._h, _slices, _ring_of), plus the circuit-breaker bits when asked,
+    in one smgx_set_fleet_state call.  The ring is per model in the reference (SelectWorkerInfo.hash_ring comes from the registry keyed by
+    model id); a call without a ring uses the model's own state with the ring cleared."""
+    model = ring.model if ring is not None else normalize_model_key(workers[0].model_id() if workers else "").encode()
+    if ring is not None and ring._h is not policy._h:
+        raise ValueError(f"hash ring belongs to another policy handle: build it with {type(policy).__name__}.hash_ring()")
+    if ring is None and model in policy._ring_of:
+        policy._h.call("smgx_hash_ring_clear", model)
+        del policy._ring_of[model]
+    urls = tuple(w.url() for w in workers)
+    if policy._slices.get(model) != urls:
+        enc = [u.encode() for u in urls]
+        arr = (C.c_char_p * max(len(enc), 1))(*enc)
+        policy._h.call("smgx_set_workers", model, arr, len(enc))
+        policy._slices[model] = urls
+    loads = _u64([w.load() for w in workers])
+    healthy = np.ascontiguousarray(np.asarray([1 if w.is_healthy() else 0 for w in workers] or [0], dtype=np.uint8))
+    circuit = None
+    if with_circuit:
+        circuit = np.ascontiguousarray(np.asarray([1 if w.circuit_breaker_can_execute() else 0 for w in workers] or [0], dtype=np.uint8))
+    policy._h.call("smgx_set_fleet_state", model, _p(loads) if len(workers) else None, _p(healthy), _p(circuit) if with_circuit else None, len(workers))
+    return model
+
+
+def _bind_ring(policy, urls, model: str) -> HashRing:
+    """The registry's per-model ring (worker/registry.rs get_hash_ring), bound to the policy's device state."""
+    ring = HashRing(urls, handle=policy._h, model=model)
+    policy._ring_of[ring.model] = ring
+    return ring
+
+
+def _seed_sequence(seed: int, call: int) -> int:
+    """The seed of a policy's call-th batch, for the policies whose reference draws from rand::rng()."""
+    return (seed + 0xD1B54A32D192ED03 * call) & (2**64 - 1)
+
+
 class PrefixHashPolicy:
     """policies::PrefixHashPolicy (prefix_hash.rs:87-235) on the GPU: XXH3 of the first N tokens → ring lookup → bounded-load check."""
 
@@ -1020,9 +1058,7 @@ class PrefixHashPolicy:
 
     def hash_ring(self, urls, model: str = UNKNOWN_MODEL_ID) -> HashRing:
         """The registry's per-model ring (worker/registry.rs get_hash_ring), bound to this policy's device state."""
-        ring = HashRing(urls, handle=self._h, model=model)
-        self._ring_of[ring.model] = ring
-        return ring
+        return _bind_ring(self, urls, model)
 
     def compute_prefix_hashes(self, requests):  # compute_prefix_hash (:106-113) for a batch
         tokens, offsets = _ragged_tokens(requests)
@@ -1032,24 +1068,7 @@ class PrefixHashPolicy:
         return out[:n]
 
     def _push_fleet(self, workers, ring: Optional[HashRing]) -> bytes:
-        # the ring is per model in the reference (SelectWorkerInfo.hash_ring comes from the registry keyed by model id); a policy
-        # without a ring for the call uses the model's own state with the ring cleared
-        model = ring.model if ring is not None else normalize_model_key(workers[0].model_id() if workers else "").encode()
-        if ring is not None and ring._h is not self._h:
-            raise ValueError("hash ring belongs to another policy handle: build it with PrefixHashPolicy.hash_ring()")
-        if ring is None and model in self._ring_of:
-            self._h.call("smgx_hash_ring_clear", model)
-            del self._ring_of[model]
-        urls = tuple(w.url() for w in workers)
-        if self._slices.get(model) != urls:
-            enc = [u.encode() for u in urls]
-            arr = (C.c_char_p * max(len(enc), 1))(*enc)
-            self._h.call("smgx_set_workers", model, arr, len(enc))
-            self._slices[model] = urls
-        loads = _u64([w.load() for w in workers])
-        healthy = np.ascontiguousarray(np.asarray([1 if w.is_healthy() else 0 for w in workers] or [0], dtype=np.uint8))
-        self._h.call("smgx_set_fleet_state", model, _p(loads) if len(workers) else None, _p(healthy), None, len(workers))
-        return model
+        return _push_ring_fleet(self, workers, ring, with_circuit=False)
 
     def select_worker_batch(self, workers, requests=None, ring: Optional[HashRing] = None, tokens=None, offsets=None, has_tokens=None):
         """One batch against one fleet snapshot → (idx int32[n] with -1 = None, branch names)."""
@@ -1145,7 +1164,7 @@ class PowerOfTwoPolicy:
 
     def next_seed(self) -> int:
         self._calls += 1
-        return (self._seed + 0xD1B54A32D192ED03 * self._calls) & (2**64 - 1)
+        return _seed_sequence(self._seed, self._calls)
 
     def select_worker_batch(self, workers, n: int, seed: Optional[int] = None, with_details: bool = False):
         """n requests against one fleet snapshot → idx int32[n] (-1 = None) [, pairs int32[n, 2], metric uint8[n]]."""
@@ -1168,6 +1187,110 @@ class PowerOfTwoPolicy:
         return None if idx[0] < 0 else int(idx[0])
 
 
+# ---- adjacent policy on the same plumbing: consistent_hashing ----------------------------------------------------------------------
+CH_HEADERS = ("x-smg-target-worker", "x-smg-routing-key", "authorization", "x-forwarded-for", "cookie")
+CH_BRANCHES = ["no_healthy_workers", "target_worker_hit", "target_worker_miss", "routing_key_hit", "random_fallback"]   # Branch::as_str
+
+
+def _ch_header_values(headers):
+    """The five values HeaderMap::get returns for CH_HEADERS (None = absent); names are case-insensitive, a repeated header (a list
+    value, or the same name twice in an item list) yields its first value."""
+    vals = [None] * len(CH_HEADERS)
+    if headers is None:
+        return vals
+    for name, v in (headers.items() if hasattr(headers, "items") else headers):
+        name = name.decode() if isinstance(name, (bytes, bytearray)) else str(name)
+        try:
+            h = CH_HEADERS.index(name.lower())
+        except ValueError:
+            continue
+        if isinstance(v, (list, tuple)):
+            if not v:
+                continue
+            v = v[0]
+        if vals[h] is None:
+            vals[h] = v.encode("utf-8") if isinstance(v, str) else bytes(v)
+    return vals
+
+
+class ConsistentHashingPolicy:
+    """policies::ConsistentHashingPolicy (consistent_hashing.rs) on the GPU: X-SMG-Target-Worker, then X-SMG-Routing-Key, then the first
+    present of authorization / x-forwarded-for / cookie hashed onto the ring (or modulo the healthy URLs without a ring), else a random
+    healthy worker.  The reference draws that worker from a thread-local generator; here every call consumes one value of a per-policy
+    seed sequence and request i of the call uses draw i of that stream."""
+
+    def __init__(self, device_id: int = 0, max_batch: int = 0, seed: int = 0x5EED):
+        self._h = _Handle(CacheAwareConfig(eviction_interval_secs=0), device_id, max_batch)
+        self._slices = {}
+        self._ring_of = {}
+        self._seed = int(seed) & (2**64 - 1)
+        self._calls = 0
+
+    def hash_ring(self, urls, model: str = UNKNOWN_MODEL_ID) -> HashRing:
+        """The registry's per-model ring (worker/registry.rs get_hash_ring), bound to this policy's device state."""
+        return _bind_ring(self, urls, model)
+
+    def next_seed(self) -> int:
+        self._calls += 1
+        return _seed_sequence(self._seed, self._calls)
+
+    def _push_fleet(self, workers, ring: Optional[HashRing]) -> bytes:
+        # the circuit-breaker bits go with the fleet although no pick reads them, so the device sees the fleet the router has
+        return _push_ring_fleet(self, workers, ring, with_circuit=True)
+
+    def name(self) -> str:  # :188-190
+        return "consistent_hashing"
+
+    def needs_request_text(self) -> bool:  # trait default (policies/mod.rs:77-79)
+        return False
+
+    def on_request_complete(self, worker_url: str, success: bool):  # trait default: no state
+        return None
+
+    def select_worker_batch(self, workers, headers_list=None, ring: Optional[HashRing] = None, seed: Optional[int] = None, with_details: bool = False,
+                            values=None, offsets=None, present=None):
+        """One batch against one fleet snapshot → idx int32[n] (-1 = None) [, branch names, key positions uint64[n]].  headers_list[i] is
+        request i's headers (a mapping, an item list, or None for info.headers = None); or pass the packed form of the C call directly:
+        values (bytes), offsets (5n + 1), present (n bit masks)."""
+        model = self._push_fleet(workers, ring)
+        seed = self.next_seed() if seed is None else int(seed) & (2**64 - 1)
+        if headers_list is not None:
+            blob, offs, present = bytearray(), [0], []
+            for hd in headers_list:
+                bits = 0
+                for h, v in enumerate(_ch_header_values(hd)):
+                    if v is not None:
+                        bits |= 1 << h
+                        blob += v
+                    offs.append(len(blob))
+                present.append(bits)
+            values, offsets = bytes(blob), offs
+        offsets = _u32(offsets)
+        present = np.ascontiguousarray(np.asarray(present, np.uint8))
+        n = present.size
+        if offsets.size != len(CH_HEADERS) * n + 1:
+            raise ValueError("offsets must hold 5 n + 1 entries")
+        vbuf = np.frombuffer(values, np.uint8) if values else np.zeros(0, np.uint8)
+        out = np.full(max(n, 1), -1, np.int32)
+        branch = np.zeros(max(n, 1), np.uint8)
+        key_pos = np.zeros(max(n, 1), np.uint64)
+        self._h.call("smgx_consistent_hashing_select_batch", model, n, _p(vbuf), _p(offsets), _p(present), seed, _p(out),
+                     _p(branch) if with_details else None, _p(key_pos) if with_details else None)
+        if with_details:
+            return out[:n], [CH_BRANCHES[b] for b in branch[:n]], key_pos[:n]
+        return out[:n]
+
+    def select_worker_impl(self, workers, info: SelectWorkerInfo):  # :116-186 → (Option<usize>, Branch)
+        idx, br, _ = self.select_worker_batch(workers, [info.headers], ring=info.hash_ring, with_details=True)
+        return (None if idx[0] < 0 else int(idx[0])), br[0]
+
+    def select_worker(self, workers, info: Optional[SelectWorkerInfo] = None) -> Optional[int]:  # LoadBalancingPolicy::select_worker (:182-186)
+        return self.select_worker_impl(workers, info or SelectWorkerInfo())[0]
+
+    def kernel_launches(self) -> int:
+        return int(self._h.L.smgx_kernel_launches(self._h.p))
+
+
 class PolicyFactory:
     """policies::PolicyFactory for the one policy this library replaces (factory.rs:17-93)."""
 
@@ -1179,6 +1302,8 @@ class PolicyFactory:
             return PrefixHashPolicy.with_defaults(**kw)
         if name.lower() in ("power_of_two", "poweroftwo"):  # factory.rs:83
             return PowerOfTwoPolicy(**kw)
+        if name.lower() in ("consistent_hashing", "consistenthashing"):  # factory.rs:87
+            return ConsistentHashingPolicy(**kw)
         return None
 
     @staticmethod
