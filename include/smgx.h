@@ -482,7 +482,16 @@ smgx_status smgx_set_load_feedback(smgx_policy* p, int enabled, char** err);
 #define SMGX_FEEDBACK_POWER_OF_TWO 4u
 smgx_status smgx_set_load_feedback_policies(smgx_policy* p, uint32_t mask, char** err);
 /* Pipelined form for the host batcher: up to smgx_pipeline_depth() submissions may be in flight; each owns a stream
- * and device staging.  Buffers must stay valid (and should be pinned) until smgx_wait(ticket) returns. */
+ * and device staging.  Buffers must stay valid (and should be pinned) until smgx_wait(ticket) returns.
+ * Each submission is decided against the index, fleet snapshot, worker slice and routing mode current when it is submitted; index and
+ * fleet changes made while it is in flight do not reach it, and tickets may be waited for in any order.  With every lane in flight a
+ * submission returns SMGX_BUSY before it changes anything (no tree insert, nothing counted).  A submission of n = 0 requests still
+ * returns a ticket.  Waiting for an unknown ticket, or a second time for the same ticket, is SMGX_INVALID_ARGUMENT.
+ * increment_processed(): the picks of an event-mode submission are credited when smgx_wait returns for its ticket (smgx_take_processed
+ * in between does not count them yet), and not at all if smgx_set_workers replaced the slice in between (it resets the counters);
+ * tree-mode submissions complete inside the call and are credited there.
+ * Load feedback with a token tree: the tree update that select_worker_min_load owes for the picks of a submission that took the
+ * imbalanced branch is applied when its ticket is waited for, so the tree receives those requests in wait order. */
 uint32_t smgx_pipeline_depth(const smgx_policy* p);
 smgx_status smgx_submit_tokens(smgx_policy* p, const char* model_key, const uint32_t* tokens, const uint32_t* offsets, uint32_t n,
                                int32_t* out_worker_idx, smgx_decision_info* out_info, uint64_t* out_ticket, char** err);

@@ -44,6 +44,7 @@ struct ModelState {
     std::vector<uint64_t> loads;
     std::vector<uint8_t> flags;      // bit0 is_healthy(), bit1 circuit_breaker_can_execute()
     std::vector<uint64_t> processed; // increment_processed() per slice index
+    uint64_t slice_version = 0;      // bumped by smgx_set_workers: a ticket credits `processed` only against the slice it was decided on
     // KvEventMonitor state for this model
     std::unique_ptr<EventIndex> indexer;
     std::unique_ptr<Tokenizer> tokenizer;   // TokenizerRegistry entry for this model
@@ -107,6 +108,7 @@ struct Lane {
     ModelState* model = nullptr;
     const int32_t* host_out = nullptr;
     uint32_t n = 0;
+    uint64_t slice_version = 0;   // ModelState::slice_version at submission
     // load-feedback bookkeeping of a host-buffer submission (see Policy::wait)
     const uint32_t* fb_tokens = nullptr;
     const uint32_t* fb_offsets = nullptr;
@@ -1066,6 +1068,7 @@ public:
         lane.model = &m;
         lane.host_out = out_idx;
         lane.n = n;
+        lane.slice_version = m.slice_version;
         lane.fb_tokens = (fb_event && m.token_tree) ? tokens : nullptr;
         lane.fb_offsets = offsets;
         lane.fb_info_host = info_host;
@@ -1077,9 +1080,11 @@ public:
             if (!l.busy || l.ticket != ticket) continue;
             SMGX_CUDA(cudaStreamSynchronize(l.stream));
             l.busy = false;
-            // increment_processed(): every event-mode / imbalanced pick increments (cache_aware.rs:437, :767, :829)
+            // increment_processed(): every event-mode / imbalanced pick increments (cache_aware.rs:437, :767, :829).  The picks index the
+            // slice of the submission: after smgx_set_workers replaced it (and reset the counters) they name no worker of the new slice.
             ModelState& m = *l.model;
-            for (uint32_t i = 0; i < l.n; ++i) {
+            const uint32_t credit = l.slice_version == m.slice_version ? l.n : 0;
+            for (uint32_t i = 0; i < credit; ++i) {
                 int32_t idx = l.host_out[i];
                 if (idx >= 0 && (size_t)idx < m.processed.size()) ++m.processed[(size_t)idx];
             }
@@ -1285,6 +1290,7 @@ smgx_status smgx_set_workers(smgx_policy* p, const char* model_key, const char* 
         m.loads.assign(n, 0);
         m.flags.assign(n, 3);
         m.processed.assign(n, 0);
+        ++m.slice_version;
         m.fleet_dirty = true;
         m.fleet_dirty_tenant = true;
         m.pf_struct_dirty = m.pf_state_dirty = true;
@@ -2592,6 +2598,7 @@ smgx_status smgx_submit_text(smgx_policy* p, const char* model_key, const uint8_
         lane.model = &m;
         lane.host_out = out_worker_idx;
         lane.n = n;
+        lane.slice_version = m.slice_version;
         *out_ticket = lane.ticket;
         return SMGX_SUCCESS;
     });
