@@ -103,7 +103,7 @@ typedef struct smgx_shard_fleet {   /* the select_worker prologue of one shard (
     int32_t first_healthy;
     uint32_t n_healthy;
     uint32_t imbalanced;     /* shard-local; the merged gate is recomputed from min_load / max_load */
-    uint64_t min_load, max_load;
+    uint64_t min_load, max_load;   /* over all the shard's workers; UINT64_MAX and 0 for a shard with no workers */
     uint64_t min_healthy_load;
 } smgx_shard_fleet;
 

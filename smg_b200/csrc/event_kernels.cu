@@ -2154,7 +2154,9 @@ __global__ void __launch_bounds__(256) fleet_prepare_kernel(FleetRaw raw, FleetD
     if (tid == 0) {
         FleetDerived d;
         uint64_t mn0 = s_mn[0] == ~0ULL ? 0 : s_mn[0], mx0 = s_mx[0];
-        d.min_load = mn0; d.max_load = mx0;
+        // min_load keeps the fold's UINT64_MAX start value for an empty slice: a worker-id shard with no workers must not lower the
+        // fleet minimum shard_reduce_kernel takes over the shards' summaries (the gate, here and there, maps UINT64_MAX to 0 like :666)
+        d.min_load = s_mn[0]; d.max_load = mx0;
         d.n_healthy = s_nh[0];
         d.min_load_idx = s_nh[0] ? s_hidx[0] : -1;
         d.first_healthy = s_nh[0] ? s_fh[0] : -1;
@@ -2616,6 +2618,7 @@ __global__ void __launch_bounds__(256) shard_reduce_kernel(const smgx_shard_cand
         n_healthy += f.n_healthy;
         if (f.n_healthy && f.min_healthy_load < hl) { hl = f.min_healthy_load; min_idx = (int32_t)(gbase[g] + (uint32_t)f.min_load_idx); }   // strict <: FIRST min
     }
+    if (mn == ~0ULL) mn = 0;   // no worker on any shard (or every load at UINT64_MAX): cache_aware.rs:666
     int32_t out = -1;
     uint32_t branch = SMGX_BR_NO_HEALTHY, matched = 0;
     if (n_healthy) {

@@ -15,7 +15,7 @@ struct FleetDerived {
     int32_t first_healthy;   // healthy_indices.first()
     uint32_t n_healthy;
     uint32_t imbalanced;     // (max-min) > abs_thr && (max as f32) > (min as f32 * rel_thr)   (cache_aware.rs:669-670)
-    uint64_t min_load, max_load;
+    uint64_t min_load, max_load;   // over ALL workers; min_load = UINT64_MAX for an empty slice (worker-id shards)
     uint64_t min_healthy_load;   // load of min_load_idx (lets worker-id shards be merged, SURVEY §8e)
 };
 static_assert(sizeof(FleetDerived) == sizeof(smgx_shard_fleet), "smgx_shard_fleet mirrors FleetDerived");

@@ -2,7 +2,10 @@
 
 Each rank owns a contiguous range of the global worker slice (so that "last max wins" keeps meaning "highest global
 index"), indexes only its own workers' KV blocks, runs the candidate kernels on the FULL request batch, and the per-request
-24-byte candidates are all-gathered and merged on every rank (smgx_shard_reduce_device).  torch.distributed is plumbing
+24-byte candidates are all-gathered and merged on every rank (smgx_shard_reduce_device).  The pick equals the reference search run
+on each shard's index alone, merged in rank order; that is the whole-fleet pick when every index entry holds workers of one prefix
+chain, but not in general (the jump search's count test and retain guard compare sizes of whole-fleet worker sets; DESIGN.md §4d
+gives a counterexample).  torch.distributed is plumbing
 here (NCCL over NVLink on a multi-GPU box, gloo when the ranks share one device); the kernels and the C ABI are the product.
 """
 import ctypes as C
