@@ -165,10 +165,11 @@ size_t TokenTreeIndex::tenant_token_size(uint32_t tenant) const {
 void TokenTreeIndex::insert_tokens(const uint32_t* toks, size_t n, uint32_t tenant) {
     const size_t aligned = (n / kPage) * kPage;
     if (aligned == 0) return;
-    if (tenant >= tenant_known_.size()) { tenant_known_.resize(tenant + 1, 0); tenant_tokens_.resize(tenant + 1, 0); }
-    if (!tenant_known_[tenant]) {   // first insert for this tenant: root entry + token counter (:412-420)
-        tenant_known_[tenant] = 1;
-        if (!has_tenant(nodes_[0], tenant)) nodes_[0].tenants.emplace_back(tenant, 0);
+    if (tenant >= tenant_known_.size()) { tenant_known_.resize(tenant + 1, 0); tenant_tokens_.resize(tenant + 1, 0); root_has_.resize(tenant + 1, 0); }
+    tenant_known_[tenant] = 1;   // token counter (:418-420)
+    if (!root_has_[tenant]) {    // root entry (:412-416), on every insert: eviction may have removed it since the first one
+        root_has_[tenant] = 1;
+        nodes_[0].tenants.emplace_back(tenant, 0);
     }
     const uint32_t* rem = toks;
     size_t rem_len = aligned;
@@ -354,6 +355,7 @@ void TokenTreeIndex::evict_tenant(uint32_t tenant, size_t max_tokens) {
         bool had = false;
         for (size_t i = 0; i < nd.tenants.size(); ++i) if (nd.tenants[i].first == tenant) { nd.tenants.erase(nd.tenants.begin() + i); had = true; break; }
         if (!had) continue;
+        if (node == 0) root_has_[tenant] = 0;
         mark_node(node);
         evicted += nd.label_len;
         uint32_t cur = node;
@@ -397,7 +399,7 @@ void TokenTreeIndex::clear() {
     table_.assign(1024, ChildSlot{0, 0, 0});
     mask_ = 1023;
     table_live_ = table_tombs_ = 0;
-    tenant_tokens_.clear(); tenant_known_.clear();
+    tenant_tokens_.clear(); tenant_known_.clear(); root_has_.clear();
     full_dirty_ = true;
     dirty_nodes_.clear(); dirty_slots_.clear();
 }

@@ -148,6 +148,7 @@ private:
     uint64_t table_live_ = 0, table_tombs_ = 0;
     std::vector<size_t> tenant_tokens_;                    // tenant_token_count (token_tree.rs:328), indexed by tenant id
     std::vector<uint8_t> tenant_known_;                    // … and whether the tenant has an entry at all
+    std::vector<uint8_t> root_has_;                        // whether the root lists the tenant (eviction can remove it)
     std::vector<uint32_t> slot_stamp_;
     uint32_t flush_gen_ = 1;
 
